@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- rays/s of the render_rays hot path (BASELINE.json metric) on N B200s.
+"""bench.py -- rays/s of the render_rays hot path (BASELINE.json metric) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--precision MODE] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--precision MODE] [--impl reference] [--dump-outputs DIR]
 
 Workload (config.workload): BASELINE.json configs[1] -- a 400x400 lego-shape frame, 160 000
 synthetic camera rays, N_samples=64 + N_importance=64, 8x256 MLP, fp32-parity arithmetic,
@@ -19,6 +19,9 @@ roofline: the fine-pass field kernel (2/3 of all FLOPs) timed alone with CUDA ev
 cpu_baseline: the CPU oracle port (the reference is Python/torch; it cannot travel to the GPU
          box) on the host cores, on a bounded sample of the same rays.
 --impl reference: only the CPU arm, same JSON schema, "impl": "reference".
+--dump-outputs DIR: after the timed steps, the render_rays outputs of the last timed step (what a caller of
+         the timed path receives) as DIR/<name>.npy, float32 (rank 0); above 64 MB in all, a fixed seeded sample
+         of rays.  Inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -40,7 +43,8 @@ FLOP_PER_POINT = 2 * 593408          # SURVEY.md 8d (full head)
 N_SAMPLES, N_IMPORTANCE = 64, 64
 POINTS_PER_RAY = N_SAMPLES + (N_SAMPLES + N_IMPORTANCE)
 METRIC = "rays/sec (64c+64f samples, 8x256 MLP)"
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+# NVIDIA data sheet, H100 SXM (700 W): used as the denominator only when MEASURED_PEAKS.json is absent
+FALLBACK_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}
 
 
 # stdout carries exactly ONE line, the JSON record: everything else that libraries write to fd 1 (NCCL's
@@ -257,7 +261,7 @@ def _timed_steps(fn, iters, flush, sync_all, dev, world):
 
 def bench_configs_2(models, emb, dev, lib, flush, sync_all, peaks):
     """BASELINE configs[2]: 504x378 LLFF shape, the 63x84 stride-4 ray patch (5 292 rays), 64+64 samples, bf16 MLP
-    operands (fp32 accumulate), one B200.  rays/s of a complete render_rays + the fine-pass field kernel alone."""
+    operands (fp32 accumulate), one GPU.  rays/s of a complete render_rays + the fine-pass field kernel alone."""
     from sinnerf_b200 import _lib, rendering, synthetic
     if lib.snb_packed_weights_bytes(_lib.PRECISIONS["bf16"]) == 0:
         return {"unavailable": "bf16 mode not built"}
@@ -408,7 +412,7 @@ def bench_configs_4_train(dev, rank, local_rank, world, precision, flush, sync_a
 
 def torch_cuda_baseline(rays_dev, default_init_params, n_prefix=8192):
     """The competitor a SinNeRF user has today (reference eval.py:141-155 on a GPU): the reference algorithm as stock
-    PyTorch ops on this B200 -- oracle/render_oracle.py (the restatement pinned to the reference) on CUDA tensors,
+    PyTorch ops on this GPU -- oracle/render_oracle.py (the restatement pinned to the reference) on CUDA tensors,
     fp32 and with allow_tf32.  Informational row; not on any product path."""
     from oracle import render_oracle as orc
     dev = rays_dev.device
@@ -441,6 +445,28 @@ def torch_cuda_baseline(rays_dev, default_init_params, n_prefix=8192):
     return out
 
 
+DUMP_LIMIT_BYTES = 60_000_000     # below 64 MB with the .npy headers
+
+
+def dump_outputs(out_dir, res):
+    """The arrays render_rays returned in the last timed step, one float32 .npy per key.  When all of them together
+    exceed DUMP_LIMIT_BYTES, the same fixed, seeded sample of rays is taken from every array (the sampled ray indices
+    are written as ray_index.npy, float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v.detach().float() for k, v in res.items() if isinstance(v, torch.Tensor) and not k.startswith("_")}
+    n = min(v.shape[0] for v in arrays.values())
+    total = sum(v.numel() * 4 for v in arrays.values())
+    idx = None
+    if total > DUMP_LIMIT_BYTES:
+        keep = int(n * (DUMP_LIMIT_BYTES - 8 * n) / total)
+        idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        np.save(os.path.join(out_dir, "ray_index.npy"), idx.double().numpy())
+    for k, v in sorted(arrays.items()):
+        v = v.cpu()
+        np.save(os.path.join(out_dir, f"{k}.npy"), (v if idx is None else v[idx]).numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -450,7 +476,11 @@ def main():
     ap.add_argument("--precision", default=os.environ.get("SINNERF_B200_BENCH_PRECISION", "auto"))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the configs[2]/[3]/[4] and stock-PyTorch rows")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     capture_stdout()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -462,7 +492,6 @@ def main():
 
     import torch.distributed as dist
     from sinnerf_b200 import _lib, synthetic
-    from sinnerf_b200 import build as _build
     from sinnerf_b200.distributed import pack_pixels, PeerPixels
     from sinnerf_b200.nerf import NeRF, Embedding
     from sinnerf_b200 import rendering
@@ -473,11 +502,7 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
-    if rank == 0:
-        _build.build()
-    if world > 1:
-        dist.barrier()
-    lib = _lib.load()
+    lib = _lib.load()          # built by __graft_entry__.build() / python -m sinnerf_b200.build
     precision = args.precision
     if precision == "auto":
         precision = "f16x3" if lib.snb_packed_weights_bytes(_lib.PRECISIONS["f16x3"]) > 0 else "fp32"
@@ -501,10 +526,12 @@ def main():
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     rendering.DRAW_UNUSED_NOISE = True     # keep the reference's randn draws (rendering.py:224)
 
+    last = {}
+
     def step(r):
         k = gather.begin() if p2p else 0
         with torch.no_grad():
-            res = rendering.render_rays(models, emb, r, N_SAMPLES, False, 0, 0, N_IMPORTANCE, 32768, True,
+            res = last["res"] = rendering.render_rays(models, emb, r, N_SAMPLES, False, 0, 0, N_IMPORTANCE, 32768, True,
                                         precision=precision, pixel_scatter=gather.scatter(k, rank * n) if p2p else None)
         pix = pack_pixels(res)
         if p2p:
@@ -547,6 +574,8 @@ def main():
     if sampler:
         sampler.start()
     total_ms = timed(lambda: step(rays_dev), args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["res"])
 
     def e2e_step():
         r = rays_pinned.to(dev, non_blocking=True)
@@ -591,25 +620,17 @@ def main():
         value = n * world / (ms_per_step / 1e3)
         e2e_value = n * world / ((e2e_ms / args.steps) / 1e3)
         kern_tflops = FLOP_PER_POINT * n * S_f / (kern_ms / 1e3) / 1e12
-        # the kernel is timed alone but in a back-to-back loop of tens of ms each: the power-capped
-        # ("sustained") cuBLAS figure is the comparable denominator
+        # a measured sustained rate (MEASURED_PEAKS.json) is the comparable denominator when present
         tensor_peak = peaks.get("bf16_tflops_sustained") or peaks.get("bf16_tflops")
         # tensor-core modes fold the 256x256 bottleneck into the direction layer at pack time, so they
         # execute (593408 - 65536) MACs per point and product; the split modes issue 3 products
         passes = (3 if precision.endswith("x3") else 1) * (593408 - 65536) / 593408
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "field_traffic.json")
-        if os.path.exists(tp):
-            try:
-                traffic = json.load(open(tp)).get(precision)
-            except Exception:
-                traffic = None
         line = {
             "metric": METRIC, "value": value, "unit": "rays/s", "n_gpus": world, "steps": args.steps,
             "warmup": max(3, args.warmup), "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None,
-            "dtype": {"fp32": "fp32 (FFMA)", "f16x3": "fp32-parity: fp16 hi/lo split x3 on tcgen05, fp32 accumulate",
-                      "bf16x3": "bf16 hi/lo split x3 on tcgen05, fp32 accumulate",
+            "dtype": {"fp32": "fp32 (FFMA)", "f16x3": "fp32-parity: fp16 hi/lo split x3 on wgmma, fp32 accumulate",
+                      "bf16x3": "bf16 hi/lo split x3 on wgmma, fp32 accumulate",
                       "bf16": "bf16 operands, fp32 accumulate"}[precision],
             "data": "synthetic",
             "config": workload_config(world, precision),
@@ -622,17 +643,16 @@ def main():
             "clocks": clocks,
             "roofline": {"bound": "tensor", "kernel": "fine-pass field kernel (160000 rays x 128 samples)",
                          "achieved": kern_tflops, "peak": tensor_peak, "unit": "TFLOP/s",
-                         "frac": kern_tflops / tensor_peak if tensor_peak else None, "traffic": traffic,
+                         "frac": kern_tflops / tensor_peak if tensor_peak else None,
                          "executed_tflops": kern_tflops * passes if precision != "fp32" else None,
                          "frac_executed": kern_tflops * passes / tensor_peak if (tensor_peak and precision != "fp32") else None,
-                         "peak_source": f"MEASURED_PEAKS.json ({peaks['_source']}), dense bf16 cuBLAS, sustained",
+                         "peak_source": ("MEASURED_PEAKS.json, dense bf16 cuBLAS, sustained" if peaks["_source"] == "measured"
+                                         else "NVIDIA data sheet, H100 SXM dense bf16 (not reached; power limit in clocks)"),
                          "ms_per_launch": kern_ms,
                          "flops": "algorithmic 2*593408 per point (SURVEY 8d); "
                                   + ("executed MMA flops: 3 products (hi*hi + hi*lo + lo*hi) x 0.89 (bottleneck folded into the dir layer)" if precision.endswith("x3")
                                      else "FFMA pipe, not tensor cores" if precision == "fp32" else "single pass")},
         }
-        line["roofline"]["traffic_source"] = ("static: dram__bytes_read+write of one ncu --set full capture of this kernel at this "
-                                              "size (profiles/field_traffic.json), not re-measured in this run")
         if extra:
             line["extra"] = extra
         if not args.no_cpu_baseline and world == 1:

@@ -19,7 +19,7 @@
  *    nothing synchronises the host;
  *  - functions return SNB_OK (0) or a negative SNB_ERR_* code; snb_last_error() returns
  *    a thread-local message for the last failing call on this thread;
- *  - the library is sm_100a only; snb_device_check() reports anything else as an error.
+ *  - the library is sm_90a (H100) only; snb_device_check() reports anything else as an error.
  */
 #ifndef SINNERF_B200_H
 #define SINNERF_B200_H
@@ -40,8 +40,8 @@ extern "C" {
 
 /* Arithmetic used for the field MLP (every other stage is always fp32).
  *  FP32     : FFMA on CUDA cores, fp32 accumulate            -- exact-fp32 mode
- *  F16X3    : tcgen05 kind::f16, operands split hi+lo (fp16), 3 products, fp32 accumulate
- *             in TMEM -- meets the <=1e-4 fp32 parity bar on tensor cores
+ *  F16X3    : wgmma f16, operands split hi+lo (fp16), 3 products, fp32 accumulate
+ *             in registers -- meets the <=1e-4 fp32 parity bar on tensor cores
  *  BF16X3   : same with bf16 halves (wider range, ~2e-5)
  *  BF16     : single-pass bf16 operands, fp32 accumulate (BASELINE.json configs[2])
  */

@@ -1,4 +1,4 @@
-"""sinnerf_b200 -- Blackwell (sm_100a) volumetric renderer behind SinNeRF's render_rays /
+"""sinnerf_b200 -- Hopper (sm_90a, H100) volumetric renderer behind SinNeRF's render_rays /
 NeRF / Embedding interface.  See DESIGN.md and INTEGRATION.md."""
 from .config import get_precision, set_precision, get_train_storage, set_train_storage  # noqa: F401
 

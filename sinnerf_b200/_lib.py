@@ -1,7 +1,7 @@
 """ctypes binding of libsinnerf_b200.so (include/sinnerf_b200.h).
 
 There is no CPU or PyTorch fallback anywhere in this package: if the shared library is missing
-or the device is not sm_100, every entry point raises.
+or the device is not sm_90 (H100), every entry point raises.
 """
 from __future__ import annotations
 
@@ -123,7 +123,7 @@ _checked_devices = set()
 
 
 def require_device(t: torch.Tensor, what: str) -> None:
-    """The product path is CUDA sm_100 only; anything else is an error, not a fallback."""
+    """The product path is CUDA sm_90 only; anything else is an error, not a fallback."""
     if not t.is_cuda:
         raise RuntimeError(f"sinnerf_b200.{what}: expected a CUDA tensor, got device '{t.device}' "
                            "(this package has no CPU path)")

@@ -1,4 +1,4 @@
-"""Process-wide settings of the sm_100a path."""
+"""Process-wide settings of the sm_90a path."""
 import os
 
 # default: the fp32-parity tensor-core mode (validated against the oracle at <= 1e-4)
@@ -6,8 +6,8 @@ _precision = os.environ.get("SINNERF_B200_PRECISION", "f16x3")
 
 
 def set_precision(name: str) -> None:
-    """Arithmetic of the field MLP: 'fp32' (FFMA, exact), 'f16x3' / 'bf16x3' (tcgen05, split operands,
-    fp32-parity), 'bf16' (tcgen05 single pass).  Everything outside the MLP is always fp32."""
+    """Arithmetic of the field MLP: 'fp32' (FFMA, exact), 'f16x3' / 'bf16x3' (wgmma, split operands,
+    fp32-parity), 'bf16' (wgmma single pass).  Everything outside the MLP is always fp32."""
     from . import _lib
     _lib.precision_id(name)
     global _precision
@@ -19,9 +19,10 @@ def get_precision() -> str:
 
 
 # Training path: how the activations the backward needs are kept.  'fp16' (default for the tensor-core modes):
-# one fp16 copy in the MMA-ready tile layout + power-of-two scaled fp16 gradients between layers (half the HBM
-# traffic and memory; parameter gradients within the 1e-3 parity bar).  'fp32': row-major fp32 activations and
-# bf16 hi/lo gradient arithmetic (round-1 kernels; the only option of precision 'fp32').
+# one fp16 copy in the MMA-ready tile layout + power-of-two scaled fp16 gradients between layers, backward on
+# tensor cores (half the HBM traffic and memory; parameter gradients within the 1e-3 parity bar).  'fp32':
+# row-major fp32 activations and the fp32-input tensor-core backward (bf16 hi/lo split; the only option of precision
+# 'fp32').  SNB_BWD_SIMT=1 runs that arm's GEMMs on the FFMA kernels instead (A/B reference).
 _train_storage = os.environ.get("SINNERF_B200_TRAIN_STORAGE", "fp16")
 
 

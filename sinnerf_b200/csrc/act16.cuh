@@ -12,13 +12,13 @@
 //   contiguous over the 32 points.  A tile is F * 64 bytes, contiguous.
 //
 //   * a warp whose lanes are 32 consecutive points writes / reads one 8-feature group as 512 contiguous
-//     bytes -- the natural pattern of the forward / dgrad epilogues (TMEM lane = point): no transposition;
-//   * a tile copied to shared memory verbatim (one cp.async.bulk) IS a tcgen05 operand in the SWIZZLE_NONE
+//     bytes; eight consecutive points of one group are 128 contiguous bytes -- the rows of a wgmma register
+//     fragment or accumulator fragment: no transposition;
+//   * a tile copied to shared memory verbatim (one cp.async.bulk) IS a wgmma operand in the SWIZZLE_NONE
 //     canonical layout: 8 points x 16 bytes = one 128-byte core matrix,
 //       - MN-major (M or N = features, K = points): LBO (K direction, next 8 points) = 128 B,
 //         SBO (MN direction, next 8 features) = 512 B          -> the wgrad contraction  dW = dY^T X
-//       - K-major  (M = points, K = features): SBO = 128 B, LBO = 512 B     (not used: dgrad keeps A in TMEM)
-//     (bit layouts validated on hardware by probes/umma_mn_probe.cu);
+//       - K-major  (M = points, K = features): SBO = 128 B, LBO = 512 B     (not used: dgrad keeps A in registers);
 //   * 2.5 KB per point and layer instead of 5 KB, and no converter warps.
 //
 // Precision: activations are post-ReLU values < 65504 (saturated), rounded to nearest fp16 (11 bits);

@@ -104,8 +104,8 @@ int snb_device_check(int* sm_count, int* cc_major, int* cc_minor) {
   if (sm_count) *sm_count = sms;
   if (cc_major) *cc_major = major;
   if (cc_minor) *cc_minor = minor;
-  if (major != 10)
-    return fail(SNB_ERR_UNSUPPORTED, "libsinnerf_b200 is built for sm_100a only; device %d is sm_%d%d", dev, major,
+  if (major != 9 || minor != 0)   // sm_90a code (wgmma) loads on compute capability 9.0 only
+    return fail(SNB_ERR_UNSUPPORTED, "libsinnerf_b200 is built for sm_90a only; device %d is sm_%d%d", dev, major,
                 minor);
   return SNB_OK;
 }

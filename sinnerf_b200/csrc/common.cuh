@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device definitions for libsinnerf_b200 (sm_100a only).
+// common.cuh -- shared host/device definitions for libsinnerf_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -134,5 +134,15 @@ __device__ __forceinline__ float widened_sigmoid_f(float x) {
   return 0.5f * (1.0f + 1.002f * tanhf(0.5f * x));
 }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
+
+// dst[0] += a (and dst[1] += b when `second`): one vector reduction when the pair is 8-byte aligned
+__device__ __forceinline__ void red_add_pair(float* dst, float a, float b, bool second) {
+  if (second && ((reinterpret_cast<uintptr_t>(dst) & 7) == 0)) {
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(a), "f"(b) : "memory");
+  } else {
+    atomicAdd(dst, a);
+    if (second) atomicAdd(dst + 1, b);
+  }
+}
 
 }  // namespace snb

@@ -1,4 +1,4 @@
-// dgrad_tc.cu -- input gradients of one nn.Linear on 5th-gen tensor cores (CTA pairs).
+// dgrad_tc.cu -- input gradients of one nn.Linear from / to fp32 row-major tensors, on Hopper tensor cores.
 //
 //   dX[p][k] = ( sum_n dY[p][n] W[n][col_off + k]  +  extra[p] evec[k] ) * [mask[p][k] > 0]        k < 256
 //
@@ -7,95 +7,66 @@
 // the layer (32 B per point, emitted by the wgrad kernel that reads that input anyway), extra/evec =
 // the sigma head's rank-1 term at h8.  dY and dX are plain row-major fp32.
 //
-// Mapping (the forward field kernel's, with HBM as the producer of A):
-//   * a CTA pair owns 256 points; tcgen05.mma.cta_group::2, M = 256, N = 128 per instruction, so the
-//     256 outputs are two halves a | b with their own TMEM accumulators: the epilogue of a runs
-//     under the MMAs of b, the epilogue of b under the next tile's a;
-//   * W^T (bf16 hi + lo, K-major canonical layout) is converted ONCE per CTA and stays resident
-//     in shared memory (128 KB: each CTA of the pair holds 64 of a half's 128 rows) -- no weight
-//     streaming at all;
-//   * the A operand lives in TMEM as bf16 hi | lo planes; eight converter warps (two per lane
-//     quadrant) read their point's dY row from HBM 32 columns at a time, split and tcgen05.st it.  Quarters form a ring with the MMA issuer: quarter q of the next tile is
-//     refilled as soon as this tile's half b has consumed it, so HBM loads stay in flight while
-//     the tensor pipe works;
-//   * bf16 3-product split (hi*hi + lo*hi + hi*lo), fp32 accumulate: gradients need fp32's range.
+// Mapping (dgrad16.cu's): CTA (x, y) owns 128-point tiles x, x + gridDim.x, ... and output columns
+// [128 y, +128); W^T of those columns is converted once to bf16 hi + lo and stays resident in shared memory
+// (128 KB at N = 256); two warpgroups (wgmma M = 64 points each, N = 128) take A from registers: each thread
+// loads its fragment's fp32 pairs (8 points of a warp read 32 contiguous bytes each), splits them into bf16
+// hi + lo and issues the register-operand wgmma.  bf16 3-product split (hi*hi + lo*hi + hi*lo), fp32
+// accumulate: gradients need fp32's range.
 //
-// HBM per point and layer: dY 4N + 32 B of mask in, dX 1 KB out (2 KB at N = 256): the kernel is
-// HBM-bound (~0.08 us per 256-point tile at 6.5 TB/s against 6144 tensor cycles); see DESIGN.md.
+// HBM per point and layer: dY 4N + 32 B of mask in, dX 1 KB out: HBM-bound.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace snb {
-using namespace umma;
+using namespace wg;
 
 namespace {
 
-constexpr int kDgTile = 128;                 // points per CTA (MMA M = 256 across the pair)
-constexpr int kDgConvWarps = 8, kDgEpiWarps = 4;      // converters: two warps per TMEM lane quadrant
-constexpr int kDgMmaWarp = kDgConvWarps + kDgEpiWarps;
-constexpr int kDgThreads = (kDgMmaWarp + 1) * 32;
-constexpr uint32_t kDgColD = 0, kDgColAhi = 256, kDgColAlo = 384;
+constexpr int kDtTile = 128;
+constexpr int kDtThreads = 256;
 
 struct DgradTcArgs {
-  const float* dY;                 // (P, NRED)
-  const float* W; int ldw; int col_off;   // nn.Linear weight (NRED, ldw); inputs [col_off, col_off + 256)
+  const float* dY;
+  const float* W; int ldw; int col_off;   // nn.Linear weight (N, ldw); inputs [col_off, col_off + 256)
   const uint32_t* mask_bits;       // (P,8) nullable: bit c of word w = [input[p][32 w + c] > 0] (wgrad_tc emits it)
   const float* extra; int extra_stride;   // nullable per-point scalar
   const float* evec;               // (256), with extra
-  float* dX;                       // (P,256)
+  float* dX;                       // (P, 256)
   long long P;
 };
 
 template <int NRED>
-struct DgSmem {
-  // W^T planes: [half a|b][hi|lo][k8 = n / 8][64 rows = this CTA's in-features of the half][8 n]
-  static constexpr int kPlaneBytes = (NRED / 8) * 64 * 16;
-  alignas(1024) unsigned char b[2][2][kPlaneBytes];
-  alignas(16) float evec[256];
-  // per-warp 32 x 32 transposition tiles (row stride 36 words: conflict-free 128-bit accesses both ways).
-  // HBM is read and written with rows-of-128-bytes per quarter warp (4 lines per instruction); the
-  // thread = point-row view TMEM wants is produced here, not by 32-lines-per-instruction global accesses.
-  alignas(16) float cstage[kDgConvWarps][32][36];
-  alignas(16) float estage[kDgEpiWarps][32][36];
-  uint64_t q_ready[4], q_free[4], d_full[2], d_drained[2];
-  uint32_t tmem_base;
+struct DtSmem {
+  // W^T planes of this CTA's 128 output columns: [hi|lo][n8][128 rows = output columns k][8 n], bf16
+  static constexpr int kPlaneBytes = (NRED / 8) * 128 * 16;
+  alignas(128) unsigned char b[2][kPlaneBytes];
+  alignas(16) float evec[128];
 };
 
 __device__ __forceinline__ void bf16_split_pair(float x0, float x1, uint32_t& hi, uint32_t& lo) {
   const __nv_bfloat162 h = __floats2bfloat162_rn(x0, x1);
   hi = *reinterpret_cast<const uint32_t*>(&h);
-  const float b0 = __uint_as_float(hi << 16), b1 = __uint_as_float(hi & 0xffff0000u);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(x0 - b0, x1 - b1);
+  const __nv_bfloat162 l = __floats2bfloat162_rn(x0 - __low2float(h), x1 - __high2float(h));
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
 template <int NRED>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kDgThreads, 1) dgrad_tc_kernel(DgradTcArgs a) {
-  using S = DgSmem<NRED>;
-  constexpr int kQ = NRED / 64;               // K quarters (64 reduction columns each)
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
+__global__ void __launch_bounds__(kDtThreads, 1) dgrad_tc_kernel(DgradTcArgs a) {
+  using S = DtSmem<NRED>;
+  constexpr int kSteps = NRED / 16;
+  extern __shared__ unsigned char smem_raw[];
   S& s = *reinterpret_cast<S*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const long long ntiles = (a.P + kDgTile - 1) / kDgTile;
-  const long long n_pairs = gridDim.x / 2, pair = blockIdx.x / 2;
-  const long long n_slots = ((ntiles + 1) / 2 + n_pairs - 1) / n_pairs;   // both CTAs run the same count
+  const int kh = blockIdx.y;
+  const long long ntiles = (a.P + kDtTile - 1) / kDtTile;
 
-  // ---------------- one-time setup: barriers, TMEM, resident W^T
-  if (tid == 0) {
-    for (int q = 0; q < 4; ++q) { mbar_init(&s.q_ready[q], kDgConvWarps * 32 * 2); mbar_init(&s.q_free[q], 1); }
-    for (int h = 0; h < 2; ++h) { mbar_init(&s.d_full[h], 1); mbar_init(&s.d_drained[h], kDgEpiWarps * 32 * 2); }
-    fence_mbar_init();
-  }
-  if (warp == kDgMmaWarp) tmem_alloc_pair(&s.tmem_base);
-  for (int i = tid; i < 256; i += kDgThreads) s.evec[i] = a.evec != nullptr ? a.evec[i] : 0.f;
-  // task = (half, n8 block, row): 8 consecutive reduction rows n of one input column k
-  for (int t = tid; t < 2 * (NRED / 8) * 64; t += kDgThreads) {
-    const int row = t & 63, n8 = (t >> 6) % (NRED / 8), half = t / (64 * (NRED / 8));
-    const int k = half * 128 + (int)rank * 64 + row;
+  for (int i = tid; i < 128; i += kDtThreads) s.evec[i] = a.evec != nullptr ? a.evec[kh * 128 + i] : 0.f;
+  for (int t = tid; t < (NRED / 8) * 128; t += kDtThreads) {
+    const int row = t & 127, n8 = t >> 7;
+    const int k = kh * 128 + row;
     uint32_t h[4], l[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -103,170 +74,97 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kDgThreads, 1) dgrad
       const float w1 = __ldg(a.W + (size_t)(n8 * 8 + 2 * j + 1) * a.ldw + a.col_off + k);
       bf16_split_pair(w0, w1, h[j], l[j]);
     }
-    const int off = n8 * (64 * 16) + row * 16;
-    *reinterpret_cast<uint4*>(s.b[half][0] + off) = make_uint4(h[0], h[1], h[2], h[3]);
-    *reinterpret_cast<uint4*>(s.b[half][1] + off) = make_uint4(l[0], l[1], l[2], l[3]);
+    const int off = n8 * (128 * 16) + row * 16;
+    *reinterpret_cast<uint4*>(s.b[0] + off) = make_uint4(h[0], h[1], h[2], h[3]);
+    *reinterpret_cast<uint4*>(s.b[1] + off) = make_uint4(l[0], l[1], l[2], l[3]);
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tbase = s.tmem_base;
-  auto tile_of = [&](long long slot) { return (pair + slot * n_pairs) * 2 + rank; };
-  // hand-offs to the MMA issuer, which lives in the leader CTA
-  auto signal = [&](uint64_t* bar) { if (!leader) mbar_arrive_remote(bar, 0); else mbar_arrive(bar); };
 
-  if (warp == kDgMmaWarp) {
-    // ======================= MMA issuer (leader CTA, one elected lane) =======================
-    if (leader && elect_one()) {
-      const uint32_t idesc = make_idesc(kFmtBF16, 2 * kDgTile, 128);
-      const uint64_t desc0 = make_smem_desc(0, 64 * 16, 128);
-      const uint32_t b_hi32 = (uint32_t)(desc0 >> 32);
-      constexpr uint32_t kStepB = (2 * 64 * 16) >> 4;      // one K16 step, in 16-byte units
-      for (long long slot = 0; slot < n_slots; ++slot) {
-        const uint32_t par = (uint32_t)slot & 1, prev = par ^ 1;
+  const int wgi = warp >> 2, wq = warp & 3, g = lane >> 2, tq = lane & 3;
+  const uint32_t bh0 = smem_u32(s.b[0]), bl0 = smem_u32(s.b[1]);
+  float acc[64];
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const long long pt0 = tile * kDtTile + wgi * 64 + wq * 16 + g;    // rows pt0 and pt0 + 8 of this thread
+    const bool in0 = pt0 < a.P, in1 = pt0 + 8 < a.P;
+    // fragments of one K16 step: (row, k 2tq..+1) and (row, k 2tq+8..+9) of rows pt0, pt0 + 8, as bf16 hi + lo
+    auto load_a = [&](int ks, uint32_t (&fh)[4], uint32_t (&fl)[4]) {
+      const int c = 16 * ks + 2 * tq;
+      const float2 z = make_float2(0.f, 0.f);
+      const float2 v0 = in0 ? __ldg(reinterpret_cast<const float2*>(a.dY + pt0 * NRED + c)) : z;
+      const float2 v1 = in1 ? __ldg(reinterpret_cast<const float2*>(a.dY + (pt0 + 8) * NRED + c)) : z;
+      const float2 v2 = in0 ? __ldg(reinterpret_cast<const float2*>(a.dY + pt0 * NRED + c + 8)) : z;
+      const float2 v3 = in1 ? __ldg(reinterpret_cast<const float2*>(a.dY + (pt0 + 8) * NRED + c + 8)) : z;
+      bf16_split_pair(v0.x, v0.y, fh[0], fl[0]);
+      bf16_split_pair(v1.x, v1.y, fh[1], fl[1]);
+      bf16_split_pair(v2.x, v2.y, fh[2], fl[2]);
+      bf16_split_pair(v3.x, v3.y, fh[3], fl[3]);
+    };
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const uint32_t d = tbase + kDgColD + h * 128;
-          const uint32_t bh = (uint32_t)desc0 + (smem_u32(s.b[h][0]) >> 4), bl = (uint32_t)desc0 + (smem_u32(s.b[h][1]) >> 4);
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    // kB K16 steps per batch, two register sets: a register-A wgmma reads its fragment asynchronously, so a set
+    // is refilled only after wgmma.wait_group has retired the batch that used it
+    constexpr int kB = 4, kBatches = kSteps / kB;
+    static_assert(kSteps % kB == 0, "K16 steps per batch");
+    uint32_t fh[2][kB][4], fl[2][kB][4];
+    auto load_batch = [&](int set, int b) {
 #pragma unroll
-          for (int q = 0; q < kQ; ++q) {
-            if (h == 0) mbar_wait(&s.q_ready[q], par);
-            if (q == 0 && slot > 0) mbar_wait(&s.d_drained[h], prev);
-            tc_fence_after();
+      for (int i = 0; i < kB; ++i) load_a(b * kB + i, fh[set][i], fl[set][i]);
+    };
+    load_batch(0, 0);
 #pragma unroll
-            for (int ks = q * 4; ks < q * 4 + 4; ++ks) {
-              const uint32_t a_hi = tbase + kDgColAhi + ks * 8, a_lo = tbase + kDgColAlo + ks * 8;
-              mma2_ts_lohi(d, a_hi, bh + ks * kStepB, b_hi32, idesc, ks > 0 ? 1u : 0u);
-              mma2_ts_lohi(d, a_lo, bh + ks * kStepB, b_hi32, idesc, 1u);
-              mma2_ts_lohi(d, a_hi, bl + ks * kStepB, b_hi32, idesc, 1u);
-            }
-            if (h == 1) mma2_commit(&s.q_free[q]);      // both halves have consumed A quarter q
-          }
-          mma2_commit(&s.d_full[h]);
-        }
+    for (int b = 0; b < kBatches; ++b) {
+      const int set = b & 1;
+      wgmma_fence();
+#pragma unroll
+      for (int i = 0; i < kB; ++i) {
+        const int ks = b * kB + i;
+        const uint64_t dbh = make_smem_desc(bh0 + ks * 2 * (128 * 16), 128 * 16, 128);
+        const uint64_t dbl = make_smem_desc(bl0 + ks * 2 * (128 * 16), 128 * 16, 128);
+        wgmma_m64n128_bf16_rs(acc, fh[set][i], dbh, ks > 0 ? 1u : 0u);
+        wgmma_m64n128_bf16_rs(acc, fl[set][i], dbh, 1u);
+        wgmma_m64n128_bf16_rs(acc, fh[set][i], dbl, 1u);
+      }
+      wgmma_commit();
+      if (b + 1 < kBatches) {
+        wgmma_wait<1>();            // batch b - 1 (the other register set) has retired
+        load_batch(set ^ 1, b + 1);
       }
     }
-    __syncwarp();
-  } else if (warp < kDgConvWarps) {
-    // ======================= converters: dY rows (HBM) -> bf16 hi | lo planes of A (TMEM) ========
-    // A unit = 32 columns of one point row (128 B).  The two warps of a quadrant take the two
-    // halves of every K quarter; the next unit's loads are issued before the current one is split
-    // and stored, so every thread keeps 128-256 B in flight (HBM latency ~1.3k cycles).
-    const int quad = warp & 3, sub = warp >> 2;
-    const uint32_t lane_base = (uint32_t)(quad * 32) << 16;
-    const long long n_units = n_slots * kQ;
-    // lane l of a load/store instruction handles 16 bytes of row (l >> 3) + 4 i, chunk l & 7
-    const int rib0 = lane >> 3, chunk = lane & 7;
-    auto load_unit = [&](long long u, float4 (&v)[8]) {
-      const long long slot = u / kQ;
-      const int q = (int)(u - slot * kQ);
-      const long long pt0 = tile_of(slot) * kDgTile + quad * 32;      // first row of this warp's block
+    wgmma_wait<0>();
+    // ---- epilogue: (+ sigma term) * mask -> dX rows
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const long long pt = pt0 + rib0 + 4 * i;
-        v[i] = (u < n_units && pt < a.P)
-                   ? __ldg(reinterpret_cast<const float4*>(a.dY + pt * NRED + q * 64 + sub * 32) + chunk)
-                   : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int rr = 0; rr < 2; ++rr) {
+      const long long pt = pt0 + 8 * rr;
+      if (pt >= a.P) continue;
+      const float ex = a.extra != nullptr ? a.extra[pt * a.extra_stride] : 0.f;
+      uint32_t mw[4] = {~0u, ~0u, ~0u, ~0u};
+      if (a.mask_bits != nullptr) {
+        const uint4 m = __ldg(reinterpret_cast<const uint4*>(a.mask_bits + pt * 8) + kh);
+        mw[0] = m.x; mw[1] = m.y; mw[2] = m.z; mw[3] = m.w;
       }
-    };
-    auto store_unit = [&](long long u, const float4 (&v)[8]) {
-      const long long slot = u / kQ;
-      const int q = (int)(u - slot * kQ);
-      float (*st)[36] = s.cstage[warp];
-      __syncwarp();                                   // the previous unit's row reads are done
+      float* dst = a.dX + pt * 256 + kh * 128;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) *reinterpret_cast<float4*>(&st[rib0 + 4 * i][chunk * 4]) = v[i];
-      __syncwarp();
-      uint32_t hi[16], lo[16];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 x = *reinterpret_cast<const float4*>(&st[lane][j * 4]);     // this thread's point row
-        bf16_split_pair(x.x, x.y, hi[2 * j], lo[2 * j]);
-        bf16_split_pair(x.z, x.w, hi[2 * j + 1], lo[2 * j + 1]);
-      }
-      if (slot > 0) { mbar_wait(&s.q_free[q], (uint32_t)(slot - 1) & 1); tc_fence_after(); }
-      tmem_st16(tbase + lane_base + kDgColAhi + q * 32 + sub * 16, hi);
-      tmem_st16(tbase + lane_base + kDgColAlo + q * 32 + sub * 16, lo);
-      tmem_wait_st();
-      tc_fence_before();
-      signal(&s.q_ready[q]);
-    };
-    {
-      float4 x[8], y[8];
-      load_unit(0, x);
-      for (long long u = 0; u < n_units; u += 2) {
-        load_unit(u + 1, y);
-        store_unit(u, x);
-        load_unit(u + 2, x);
-        if (u + 1 < n_units) store_unit(u + 1, y);
-      }
-    }
-  } else {
-    // ======================= epilogue: D (TMEM) -> (+ sigma term) * mask -> dX (HBM) ===========
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(quad * 32) << 16;
-    const int rib0 = lane >> 3, chunk = lane & 7;
-    float (*st)[36] = s.estage[warp - kDgConvWarps];
-    for (long long slot = 0; slot < n_slots; ++slot) {
-      const long long pt0 = tile_of(slot) * kDgTile + quad * 32;
-      const long long pt = pt0 + lane;
-      const bool live = pt < a.P;
-      const float ex = (live && a.extra != nullptr) ? a.extra[pt * a.extra_stride] : 0.f;
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        uint4 mb = make_uint4(~0u, ~0u, ~0u, ~0u);
-        if (live && a.mask_bits != nullptr) mb = __ldg(reinterpret_cast<const uint4*>(a.mask_bits + pt * 8) + h);
-        const uint32_t mw[4] = {mb.x, mb.y, mb.z, mb.w};
-        mbar_wait(&s.d_full[h], (uint32_t)slot & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int c0 = h * 128 + g * 32;
-          uint32_t v[32];
-          tmem_ld32(tbase + lane_base + kDgColD + c0, v);
-          tmem_wait_ld();
-          if (g == 3) { tc_fence_before(); signal(&s.d_drained[h]); }   // half h is in registers
-          __syncwarp();                                   // the previous group's tile has been written out
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 e = *reinterpret_cast<const float4*>(s.evec + c0 + 4 * j);
-            float4 o;
-            o.x = (mw[g] >> (4 * j)) & 1u ? fmaf(ex, e.x, __uint_as_float(v[4 * j])) : 0.f;
-            o.y = (mw[g] >> (4 * j + 1)) & 1u ? fmaf(ex, e.y, __uint_as_float(v[4 * j + 1])) : 0.f;
-            o.z = (mw[g] >> (4 * j + 2)) & 1u ? fmaf(ex, e.z, __uint_as_float(v[4 * j + 2])) : 0.f;
-            o.w = (mw[g] >> (4 * j + 3)) & 1u ? fmaf(ex, e.w, __uint_as_float(v[4 * j + 3])) : 0.f;
-            *reinterpret_cast<float4*>(&st[lane][j * 4]) = o;
-          }
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const long long pr = pt0 + rib0 + 4 * i;
-            if (pr < a.P)
-              *(reinterpret_cast<float4*>(a.dX + pr * 256 + c0) + chunk) = *reinterpret_cast<const float4*>(&st[rib0 + 4 * i][chunk * 4]);
-          }
-        }
+      for (int j = 0; j < 16; ++j) {
+        const int c = 8 * j + 2 * tq;
+        const float2 e = *reinterpret_cast<const float2*>(s.evec + c);
+        const float x0 = (mw[c >> 5] >> (c & 31)) & 1u ? fmaf(ex, e.x, acc[4 * j + 2 * rr]) : 0.f;
+        const float x1 = (mw[c >> 5] >> ((c & 31) + 1)) & 1u ? fmaf(ex, e.y, acc[4 * j + 2 * rr + 1]) : 0.f;
+        *reinterpret_cast<float2*>(dst + c) = make_float2(x0, x1);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();     // neither CTA leaves (or frees TMEM) while its peer may still touch it
-  if (warp == kDgMmaWarp) tmem_dealloc_pair(tbase);
 }
 
 template <int NRED>
 int launch_dgrad_tc(const DgradTcArgs& a, cudaStream_t st) {
   static SmemOptIn optin;
-  const int smem = (int)sizeof(DgSmem<NRED>) + 1024;
+  const int smem = (int)sizeof(DtSmem<NRED>) + 1024;
   if (int rc = ensure_smem(dgrad_tc_kernel<NRED>, optin, smem, "dgrad_tc")) return rc;
-  const int sms = sm_count();
-  const long long ntiles = (a.P + kDgTile - 1) / kDgTile;
-  long long pairs = (ntiles + 1) / 2;
-  if (pairs > sms / 2) pairs = sms / 2;
-  dgrad_tc_kernel<NRED><<<(unsigned)(2 * pairs), kDgThreads, smem, st>>>(a);
+  const long long ntiles = (a.P + kDtTile - 1) / kDtTile;
+  long long ctas = (sm_count() + 1) / 2;          // two column halves per tile
+  if (ctas > ntiles) ctas = ntiles;
+  dgrad_tc_kernel<NRED><<<dim3((unsigned)ctas, 2), kDtThreads, smem, st>>>(a);
   return check_launch("dgrad_tc_kernel");
 }
 

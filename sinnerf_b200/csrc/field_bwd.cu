@@ -327,7 +327,7 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(HeadArgs a) {
 // ------------------------------------------------------------------------------------------
 static int dev_sms() { return sm_count(); }
 
-// wgrad_tc.cu: the same contraction on tensor cores (bf16 hi/lo split, fp32 accumulate in TMEM)
+// wgrad_tc.cu: the same contraction on tensor cores (wgmma, bf16 hi/lo split, fp32 accumulate in registers)
 int run_wgrad_tc(const float* dY, int N, const float* X, int ldx, int K, float* dW, int ldw, int col_off, float* db,
                  uint32_t* x_pos_bits, long long P, cudaStream_t st);
 

@@ -1,53 +1,37 @@
-// field_tc.cu -- the fused field pass on 5th-gen tensor cores (tcgen05 / TMEM / bulk TMA).
+// field_tc.cu -- the fused field pass on Hopper tensor cores (wgmma / bulk TMA / mbarrier).
 //
 // Same contract as field_simt.cu (points o+d*z, both positional encodings, the 12-layer MLP,
 // [r,g,b,sigma] out; reference models/rendering.py:184-212,284-285 + models/nerf.py:24-41,
-// 105-148), but every 256-wide layer is a chain of tcgen05.mma instructions:
+// 105-148), but every 256-wide layer is a chain of wgmma.mma_async instructions:
 //
-//   * persistent CTA PAIRS (cluster of 2, cta_group::2): every MMA is M = 256 -- 128 points of
-//     the even CTA's tile and 128 of the odd CTA's -- and each CTA stages only HALF of every
-//     weight chunk.  Measured reason: an SM ingests ~28 B/clk from L2, and a 1-CTA design needs
-//     2.3 MB of weights per 128-point tile, i.e. 84k cycles of ingest against 56k cycles of MMA;
-//     the pair halves the bytes per SM (probes/umma2_probe.cu validated the 2-CTA forms);
-//   * accumulator D (128 x 256 fp32) in TMEM columns [0,256);
-//   * the NEXT layer's A operand never touches shared memory or HBM: the epilogue warps read
-//     D with tcgen05.ld, add bias, apply ReLU, split the fp32 value into a 16-bit hi part and a
-//     16-bit lo part and write both back to TMEM columns [256,384) / [384,512) with tcgen05.st;
-//     the MMAs read A straight from TMEM (".ts" operand form);
-//   * weights stream from L2 through a 5-stage smem ring of 32 KB chunk shares (per CTA: 64 output
-//     rows x 128 K x {hi,lo}) with cp.async.bulk (1-D TMA) + mbarrier complete_tx; the packed image is laid
-//     out in exactly the order the MMA warp consumes it, in the SWIZZLE_NONE K-major canonical
-//     core-matrix layout, so one share is one contiguous run of copies;
-//   * one elect.sync-elected lane runs the whole MMA-issuer role over a schedule unrolled at compile
-//     time (35 chunks per tile; every wait, operand offset and commit is an immediate): the tensor
-//     queue is 20+ instructions deep and an MMA costs ~10 issue cycles (probes/umma_issue_probe.cu),
-//     so a lean issuer stays ahead of the pipe; a table-driven loop (~200 instructions per chunk) did not;
-//   * fp32 parity (SNB_PREC_F16X3 / BF16X3): x*w ~= xh*wh + xl*wh + xh*wl, three MMAs per K
-//     step with fp32 accumulation -- 22 (fp16) or 16 (bf16) significand bits per operand;
+//   * persistent CTAs of two warpgroups; a CTA works on 128-point tiles,
+//     each warpgroup owns 64 of the rows (wgmma M = 64) and both share one weight stream, so every
+//     weight byte a CTA ingests from L2 feeds 128 points;
+//   * a layer's whole 64 x 256 fp32 accumulator lives in registers (two N = 128 halves, 128 registers
+//     per thread); the epilogue adds the bias, applies ReLU, splits the value into a 16-bit hi part and
+//     a 16-bit lo part and writes both into shared memory in the SWIZZLE_NONE K-major canonical layout,
+//     where the next layer's wgmmas read them as the A operand;
+//   * weights stream from L2 through a shared-memory ring of chunks (128 output rows x 32 K x {hi, lo})
+//     with cp.async.bulk (1-D TMA) + mbarrier complete_tx; the packed image is laid out in exactly the
+//     order the warpgroups consume it, in the same canonical layout, so a chunk is one contiguous copy;
+//   * fp32 parity (SNB_PREC_F16X3 / BF16X3): x*w ~= xh*wh + xl*wh + xh*wl, three wgmmas per K step
+//     with fp32 accumulation -- 22 (fp16) or 16 (bf16) significand bits per operand;
 //     SNB_PREC_BF16 is the single product;
-//   * positional encodings (63->64, 27->32 columns) are computed by the epilogue warps into
-//     shared memory in the canonical layout and consumed by ".ss" MMAs at layers 1, 5 (skip)
-//     and the direction layer, so neither concat exists;
-//   * sigma (256->1) and rgb (128->3) heads are fp32 dot products inside the epilogue;
+//   * positional encodings (63->64, 27->32 columns) are computed into shared memory in the canonical
+//     layout at the start of a tile and consumed at layers 1, 5 (skip) and the direction layer, so
+//     neither concat exists;
+//   * sigma (256->1) and rgb (128->3) heads are fp32 dot products inside the epilogue (quad shuffles
+//     combine the columns a thread's neighbours hold);
 //   * the bottleneck layer (256->256, no activation, nerf.py:140) is folded into the direction layer at
 //     pack time: Wd[:, :256] (Wf h + bf) = (Wd[:, :256] Wf) h + Wd[:, :256] bf -- one 256-wide layer
 //     (11 % of the MMA work) less per point, same function up to fp32 rounding.
 //
-// Schedule inside a layer (N = 256 split in halves a|b, K = 256 in halves 0|1):
-//     (a,k0) (a,k1) -> D_a full | (b,k0) -> A[k0] free | (b,k1) -> D_b full
-// Epilogue a (reads D_a, writes the next layer's A[k0]) overlaps both b phases -- it only has to
-// hold its stores until (b,k0), the last reader of A[k0], has retired; epilogue b overlaps the
-// next layer's (a,k0).  Measured with the clock64 trace (tools/trace_field.py): an epilogue half
-// costs ~1400 cycles against 1536 per MMA phase, so the older interleaved order stalled ~1000
-// cycles per layer.
-//
-// kTrain (snb_field_forward_train): the same kernel also writes the embeddings and every layer's
-// post-activation output (fp32, row-major) for the backward; those stores go through per-warp
-// shared-memory transposition tiles so that they leave as 64-byte runs, and the weight ring shrinks
-// to 3 stages to make room.
+// kTrain (snb_field_forward_train / _train16): the same kernel also writes the embeddings and every
+// layer's post-activation output for the backward -- fp32 row-major (kTrain = 1) or fp16 cells of the
+// T32 layout + ReLU mask words (kTrain = 2, act16.cuh).
 //
 // Roofline: tensor pipe.  Executed MMA FLOPs are 3x the algorithmic 1 186 816 FLOP/point in the
-// split modes.  HBM traffic: 4 B/point in (z) + 16 B/point out; weights (2.3 MB per tile pass)
+// split modes.  HBM traffic: 4 B/point in (z) + 16 B/point out; weights (2.2 MB per tile pass)
 // are L2 hits.
 #include <stdlib.h>
 
@@ -56,39 +40,20 @@
 
 #include "act16.cuh"
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace snb {
-using namespace umma;
+using namespace wg;
 
 // ------------------------------------------------------------------ geometry
-constexpr int kTile = 128;             // points per CTA tile (MMA M = 128 * cta_group)
-constexpr int kNh = 128;               // output columns per MMA (N); a 256-wide layer is two halves
-constexpr int kEpiWarps = 16;          // warps 0..15: prologue / epilogue (4 per TMEM lane quadrant)
-constexpr int kMmaWarp = 16, kLoadWarp = 17;
-constexpr int kEncWarp0 = 18, kEncWarps = 2;   // positional encodings of the NEXT slot, off the epilogue warps' critical path
-constexpr int kThreads = (kEncWarp0 + kEncWarps) * 32;   // 640: <= 102 registers per thread (96 used)
-constexpr uint32_t kColD = 0, kColAhi = 256, kColAlo = 384;
-
-// per cta_group geometry: a chunk is 128 output rows x (16 * steps) of K, steps <= kMaxSteps; each
-// CTA of the group holds kRowsB = 128 / cg of those rows
-template <int kCg>
-struct Geo {
-  static constexpr int kKc = kCg == 2 ? 128 : 32;            // K per full chunk
-  static constexpr int kRowsB = kNh / kCg;
-  static constexpr int kMaxSteps = kKc / 16;
-  static constexpr uint32_t kStepBytes = kRowsB * 16 * 2;    // one K16 step of one of {hi, lo} of a CTA's share
-  static constexpr uint32_t kPartBytesMax = kStepBytes * kMaxSteps;
-};
+constexpr int kTile = 128;             // points per CTA tile
+constexpr int kNh = 128;               // output columns per wgmma (N); a 256-wide layer is two halves
+constexpr int kKc = 32;                // K per weight chunk
+constexpr uint32_t kStepBytes = kNh * 16 * 2;   // one K16 step of one of {hi, lo} of a chunk
+constexpr int kWgs = 2;                // warpgroups, 64 tile rows each
+constexpr int kThreads = kWgs * 128;
 
 enum { SRC_ENC = 0, SRC_HID = 1, SRC_DIR = 2 };
-// WAIT_A0..A3: the previous layer's epilogue has stored output columns [64q, 64q+64) (= this layer's K
-// quarter q) into the A operand -- and the threads that own those columns have read them out of the
-// accumulator.  An MMA with accumulate = 0 overwrites all 128 columns of its half, so the first chunk on
-// half a waits for A0 AND A1 (both column quarters of D_a drained), not just for the quarter whose data it
-// consumes first; half b's first chunk comes after (a,k1), which has waited for A2 and A3.
-enum { WAIT_NONE = 0, WAIT_ENC = 1, WAIT_DIR = 2, WAIT_A0 = 4, WAIT_A1 = 5, WAIT_A2 = 6, WAIT_A3 = 7 };
-enum { COMMIT_NONE = 0, COMMIT_D0 = 1, COMMIT_D1 = 2, COMMIT_AFREE = 4 };   // bit flags
 
 struct alignas(16) Chunk {
   uint8_t layer;     // 0..9 (8 = bottleneck, 9 = direction layer)
@@ -98,11 +63,7 @@ struct alignas(16) Chunk {
   uint8_t w16;       // K offset in the layer's padded weight K space (gemm_k), in K16 steps
   uint8_t steps;     // K16 steps in this chunk
   uint8_t first;     // first chunk of this (layer, half): accumulate = 0
-  uint8_t wait;      // WAIT_* before the first step
-  uint8_t wait_mid;  // WAIT_* before step `mid` (a chunk that spans two K quarters)
-  uint8_t mid;       // first step of the second part (== steps when there is no second part)
-  uint8_t commit;    // COMMIT_* flags after issuing
-  uint8_t wait2;     // second WAIT_* before the first step (a chunk that overwrites accumulator half a)
+  uint8_t pad;
   uint16_t off;      // K16 steps of all earlier chunks: byte offset in the image = off * step bytes
   uint16_t pad2;
 };
@@ -114,9 +75,7 @@ struct ChunkTable {
   int steps_total;   // sum of steps
 };
 
-// order inside a layer: half a (enc, hid k 0..255) -> D_a | half b (enc, hid k 0..127) -> A[k0] free |
-// (hid k 128..255) -> D_b
-template <int KC>
+// order inside a layer: half a (enc, hid, dir segments in K order) | half b (same)
 __host__ __device__ constexpr ChunkTable make_chunk_table() {
   ChunkTable t{};
   int n = 0, off = 0;
@@ -132,33 +91,11 @@ __host__ __device__ constexpr ChunkTable make_chunk_table() {
         const int src = seg == 0 ? SRC_ENC : (seg == 1 ? SRC_HID : SRC_DIR);
         const int klen = seg == 0 ? (has_enc ? kXyzPad : 0) : (seg == 1 ? (has_hid ? kWidth : 0) : (l == 9 ? kDirPad : 0));
         const int wbase = seg == 0 ? 0 : (seg == 1 ? (has_enc ? kXyzPad : 0) : kWidth);   // padded weight K offset
-        for (int k0 = 0; k0 < klen; k0 += KC) {
-          const int kc = klen - k0 < KC ? klen - k0 : KC;
+        for (int k0 = 0; k0 < klen; k0 += kKc) {
+          const int kc = klen - k0 < kKc ? klen - k0 : kKc;
           Chunk c{};
           c.layer = l; c.half = half; c.src = src; c.a16 = k0 / 16; c.w16 = (wbase + k0) / 16; c.steps = kc / 16;
-          c.first = first; c.mid = c.steps; c.off = off;
-          int w = WAIT_NONE, w2 = WAIT_NONE, wm = WAIT_NONE;
-          if (src == SRC_ENC && half == 0) {
-            w = (l == 0) ? WAIT_ENC : WAIT_A0;                 // skip layer: D_a drained = both of its quarters
-            if (l != 0) w2 = WAIT_A1;
-          }
-          if (src == SRC_DIR) w = WAIT_DIR;
-          if (src == SRC_HID && half == 0) {
-            // half a consumes K quarters 2 and 3 as the previous layer's epilogue delivers them; quarters 0
-            // and 1 are both needed before the first (accumulator-overwriting) MMA of the half
-            if (k0 == 0) {
-              if (!has_enc) { w = WAIT_A0; w2 = WAIT_A1; }
-            } else {
-              if (k0 % 64 == 0) w = WAIT_A0 + k0 / 64;
-              if (kc > 64) { wm = WAIT_A0 + k0 / 64 + 1; c.mid = (64 - k0 % 64) / 16; }
-            }
-          }
-          c.wait = w; c.wait2 = w2; c.wait_mid = wm;
-          const bool last_of_half = (seg == 2) || (seg == 1 && k0 + kc == klen && l != 9) || (seg == 0 && !has_hid && k0 + kc == klen);
-          if (last_of_half) c.commit = half == 0 ? COMMIT_D0 : COMMIT_D1;
-          // the last reader of A[k 0..127] in this layer: half b's chunk ending at K = 128
-          if (half == 1 && seg == 1 && k0 + kc == 128) c.commit |= COMMIT_AFREE;
-          if (half == 1 && !has_hid && last_of_half) c.commit |= COMMIT_AFREE;
+          c.first = first; c.off = off;
           t.c[n++] = c;
           off += c.steps;
           first = false;
@@ -171,42 +108,10 @@ __host__ __device__ constexpr ChunkTable make_chunk_table() {
   t.steps_total = off;
   return t;
 }
-__constant__ ChunkTable c_chunks_cg2 = make_chunk_table<128>();
-static constexpr ChunkTable h_chunks_cg2 = make_chunk_table<128>();
-static_assert(h_chunks_cg2.n_total == 35 && h_chunks_cg2.n_sigma_only == 32, "chunk schedule (K128)");
-static_assert(h_chunks_cg2.steps_total == 258, "K16 steps per tile");
-template <int kCg>
-__device__ __forceinline__ const ChunkTable& chunk_table() {
-  static_assert(kCg == 2, "only CTA pairs are built");
-  return c_chunks_cg2;
-}
-
-// number of waits on barrier code `code` (WAIT_*) in chunks [0, ci) -- plus chunk ci's own `wait` when
-// the question is about its mid-chunk wait.  a_ready[q] completes once per layer epilogue, 8 per
-// slot, so (prior_waits & 1) is the parity to wait for.
-// stage: 0 = the chunk's first pre-wait, 1 = its second pre-wait, 2 = its mid-chunk wait
-__host__ __device__ constexpr int prior_waits(const ChunkTable& t, int ci, int code, int stage) {
-  int n = 0;
-  for (int i = 0; i < ci; ++i) n += (t.c[i].wait == code) + (t.c[i].wait2 == code) + (t.c[i].wait_mid == code);
-  if (stage >= 1) n += t.c[ci].wait == code;
-  if (stage >= 2) n += t.c[ci].wait2 == code;
-  return n;
-}
-__host__ __device__ constexpr bool wait_counts_ok(const ChunkTable& t) {
-  for (int q = 0; q < 4; ++q) {
-    if (prior_waits(t, t.n_total, WAIT_A0 + q, 0) != 8) return false;       // layers 1..7 and the dir layer
-    if (prior_waits(t, t.n_sigma_only, WAIT_A0 + q, 0) != 7) return false;  // + the explicit drain of layer 8's
-  }
-  return prior_waits(t, t.n_total, WAIT_ENC, 0) == 1 && prior_waits(t, t.n_total, WAIT_DIR, 0) == 1;
-}
-static_assert(wait_counts_ok(h_chunks_cg2), "static wait parities");
-
-template <class F, int... I>
-__device__ __forceinline__ void static_for_impl(F&& f, std::integer_sequence<int, I...>) {
-  (f(std::integral_constant<int, I>{}), ...);
-}
-template <int N, class F>
-__device__ __forceinline__ void static_for(F&& f) { static_for_impl(f, std::make_integer_sequence<int, N>{}); }
+__constant__ ChunkTable c_chunks = make_chunk_table();
+static constexpr ChunkTable h_chunks = make_chunk_table();
+static_assert(h_chunks.n_total == 129 && h_chunks.n_sigma_only == 120, "chunk schedule (K32)");
+static_assert(h_chunks.steps_total == 258, "K16 steps per tile");
 
 // ------------------------------------------------------------------ packed image
 // [PackedHeader 256 B][consts: biases + head weights, fp32][chunk 0][chunk 1]...
@@ -229,18 +134,25 @@ constexpr int kConstFloats = make_const_layout().total;
 constexpr size_t kConstBytes = (size_t)kConstFloats * 4;
 
 __host__ __device__ constexpr bool prec_split(int precision) { return precision != SNB_PREC_BF16; }
-// image bytes of one K16 step of a chunk (all CTAs' shares, hi and lo): 128 rows x 16 K x 2 B (x2)
+// image bytes of one K16 step of a chunk (hi and lo): 128 rows x 16 K x 2 B (x2)
 __host__ __device__ constexpr uint32_t step_image_bytes(int precision) {
   return (uint32_t)(kNh * 16 * 2 * (prec_split(precision) ? 2 : 1));
 }
 // scratch at the end of the image: W' = Wd[:, :256] Wf (128 x 256) and b' = bd + Wd[:, :256] bf (128)
 constexpr size_t kFusedFloats = (size_t)kHalf * kWidth + kHalf;
 __host__ __device__ constexpr size_t chunks_bytes(int precision) {
-  return (size_t)make_chunk_table<128>().steps_total * step_image_bytes(precision);
+  return (size_t)make_chunk_table().steps_total * step_image_bytes(precision);
 }
 size_t tc_packed_bytes(int precision) {
   return sizeof(PackedHeader) + kConstBytes + chunks_bytes(precision) + kFusedFloats * sizeof(float);
 }
+
+template <class F, int... I>
+__device__ __forceinline__ void static_for_impl(F&& f, std::integer_sequence<int, I...>) {
+  (f(std::integral_constant<int, I>{}), ...);
+}
+template <int N, class F>
+__device__ __forceinline__ void static_for(F&& f) { static_for_impl(f, std::make_integer_sequence<int, N>{}); }
 
 // 16-bit conversions -------------------------------------------------------------------
 template <bool kBf16>
@@ -330,9 +242,8 @@ __device__ __forceinline__ float softplus_fast(float s) {
 
 // sin / cos for the positional encoding of the single-product bf16 mode: two-constant Cody-Waite reduction to
 // [-pi, pi] and the MUFU approximations (abs error ~1e-6 for |x| up to ~1e4 -- three orders below bf16's 2^-9
-// rounding of the encoded value), ~8 instructions instead of sincosf's ~50.  In that mode an MMA phase is only 512
-// cycles and the encoding, done by the epilogue warps between layers, was on the critical path: 8.8k of a 32k-cycle
-// slot (profiles/r02_trace_bf16_before_fast_trig.txt).  The fp32-parity modes keep the accurate sincosf.
+// rounding of the encoded value), ~8 instructions instead of sincosf's ~50; the encoding of a tile sits between two
+// tiles' MMAs.  The fp32-parity modes keep the accurate sincosf.
 __device__ __forceinline__ void sincos_fast(float x, float* sn, float* cs) {
   const float k = rintf(x * 0.15915494309189535f);
   float r = fmaf(k, -6.2831854820251465f, x);
@@ -340,7 +251,6 @@ __device__ __forceinline__ void sincos_fast(float x, float* sn, float* cs) {
   *sn = __sinf(r);
   *cs = __cosf(r);
 }
-
 // ------------------------------------------------------------------ pack kernel
 using ParamPtrsTc = ParamPtrs;
 
@@ -360,11 +270,10 @@ __global__ void fuse_bottleneck_kernel(ParamPtrsTc pp, float* fused, const Packe
   }
 }
 
-template <bool kBf16, bool kSplit, int kCg>
+template <bool kBf16, bool kSplit>
 __global__ void pack_tc_kernel(ParamPtrsTc pp, int precision, int new_activation, unsigned char* image, int only_if_dirty) {
-  using G = Geo<kCg>;
   constexpr ConstLayout CL = make_const_layout();
-  const ChunkTable& tab = chunk_table<kCg>();
+  const ChunkTable& tab = c_chunks;
   PackedHeader* hdr = reinterpret_cast<PackedHeader*>(image);
   if (only_if_dirty && !hdr->dirty) return;
   float* cst = reinterpret_cast<float*>(image + sizeof(PackedHeader));
@@ -375,7 +284,7 @@ __global__ void pack_tc_kernel(ParamPtrsTc pp, int precision, int new_activation
     hdr->magic = kMagic;
     hdr->precision = precision;
     hdr->new_activation = new_activation;
-    hdr->cta_group = kCg;
+    hdr->cta_group = 1;
   }
   for (int e = gtid; e < kConstFloats; e += gsz) {
     float v = 0.f;
@@ -389,8 +298,8 @@ __global__ void pack_tc_kernel(ParamPtrsTc pp, int precision, int new_activation
     else if (e >= CL.rgb_b && e < CL.rgb_b + 3) v = pp.p[kRgbB][e - CL.rgb_b];
     cst[e] = v;
   }
-  // chunk image: [CTA 0 share: hi | lo][CTA 1 share: hi | lo]; each of hi / lo is the canonical
-  // (SWIZZLE_NONE, K-major) block [k8][kRowsB rows][8 elements] of the chunk's 16*steps K columns
+  // chunk image: [hi | lo]; each of hi / lo is the canonical (SWIZZLE_NONE, K-major) block
+  // [k8][128 rows][8 elements] of the chunk's 16*steps K columns
   constexpr int kParts = kSplit ? 2 : 1;
   const int total = tab.steps_total * kNh * 16;
   for (int e = gtid; e < total; e += gsz) {
@@ -407,10 +316,9 @@ __global__ void pack_tc_kernel(ParamPtrsTc pp, int precision, int new_activation
     const int src_k = l == 0 ? 63 : (l == 4 ? 319 : (l == 9 ? 283 : 256));
     float w = col >= 0 ? pp.p[param_weight_index(l)][n * src_k + col] : 0.f;
     if (l == 9 && kpad < kWidth) w = fused[n * kWidth + kpad];     // direction layer sees h8 through W'
-    const int owner = r / G::kRowsB, rr = r - owner * G::kRowsB;
-    const uint32_t part = G::kStepBytes * c.steps;                // bytes of one of {hi, lo} of a share
-    unsigned char* base = chunks + (size_t)c.off * (G::kStepBytes * kParts * kCg) + (size_t)owner * part * kParts;
-    const uint32_t off = (uint32_t)(kk >> 3) * (G::kRowsB * 16) + rr * 16 + (kk & 7) * 2;
+    const uint32_t part = kStepBytes * c.steps;                   // bytes of one of {hi, lo} of a chunk
+    unsigned char* base = chunks + (size_t)c.off * (kStepBytes * kParts);
+    const uint32_t off = (uint32_t)(kk >> 3) * (kNh * 16) + r * 16 + (kk & 7) * 2;
     if (kSplit) {
       uint16_t hi, lo;
       split16<kBf16>(w, hi, lo);
@@ -422,60 +330,35 @@ __global__ void pack_tc_kernel(ParamPtrsTc pp, int precision, int new_activation
   }
 }
 
-template <int kCg>
-static int launch_pack_tc_cg(const ParamPtrsTc& pp, int precision, int new_activation, unsigned char* img,
-                             int only_if_dirty, cudaStream_t st) {
-  if (precision < SNB_PREC_F16X3 || precision > SNB_PREC_BF16)
-    return fail(SNB_ERR_INVALID, "launch_pack_tc: precision %d is not a tensor-core mode", precision);
-  float* fused = reinterpret_cast<float*>(img + sizeof(PackedHeader) + kConstBytes + chunks_bytes(precision));
-  fuse_bottleneck_kernel<<<148, 256, 0, st>>>(pp, fused, reinterpret_cast<const PackedHeader*>(img), only_if_dirty);
-  if (int rc = check_launch("fuse_bottleneck_kernel")) return rc;
-  if (precision == SNB_PREC_F16X3) pack_tc_kernel<false, true, kCg><<<296, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
-  else if (precision == SNB_PREC_BF16X3) pack_tc_kernel<true, true, kCg><<<296, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
-  else if (precision == SNB_PREC_BF16) pack_tc_kernel<true, false, kCg><<<296, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
-  else return fail(SNB_ERR_INVALID, "launch_pack_tc: precision %d is not a tensor-core mode", precision);
-  return check_launch("pack_tc_kernel");
-}
-
 int launch_pack_tc(const float* const* params, int precision, int new_activation, void* image, int only_if_dirty,
                    cudaStream_t st) {
   ParamPtrsTc pp;
   for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) pp.p[i] = params[i];
   unsigned char* img = reinterpret_cast<unsigned char*>(image);
-  return launch_pack_tc_cg<2>(pp, precision, new_activation, img, only_if_dirty, st);
+  if (precision < SNB_PREC_F16X3 || precision > SNB_PREC_BF16)
+    return fail(SNB_ERR_INVALID, "launch_pack_tc: precision %d is not a tensor-core mode", precision);
+  float* fused = reinterpret_cast<float*>(img + sizeof(PackedHeader) + kConstBytes + chunks_bytes(precision));
+  fuse_bottleneck_kernel<<<132, 256, 0, st>>>(pp, fused, reinterpret_cast<const PackedHeader*>(img), only_if_dirty);
+  if (int rc = check_launch("fuse_bottleneck_kernel")) return rc;
+  if (precision == SNB_PREC_F16X3) pack_tc_kernel<false, true><<<264, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
+  else if (precision == SNB_PREC_BF16X3) pack_tc_kernel<true, true><<<264, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
+  else pack_tc_kernel<true, false><<<264, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
+  return check_launch("pack_tc_kernel");
 }
 
 // ------------------------------------------------------------------ shared memory
-// kTrain: 0 = inference, 1 = training forward keeping fp32 row-major activations (snb_field_forward_train),
-//         2 = training forward keeping fp16 activations in the T32 layout + ReLU mask words (act16.cuh)
-template <bool kSplit, int kCg, int kTrain = 0>
+template <bool kSplit>
 struct TcSmem {
   static constexpr int kParts = kSplit ? 2 : 1;
-  static constexpr uint32_t kStageBytes = Geo<kCg>::kPartBytesMax * kParts;   // this CTA's share of a full chunk
-  // up to 160 KB of weights in flight; the training forward gives 64 KB of that to the store tiles below
-  static constexpr int kStagesRaw = ((kTrain == 1 ? 96 : 160) * 1024) / kStageBytes;
-  static constexpr int kStages = kStagesRaw > 16 ? 16 : kStagesRaw;
-  alignas(1024) unsigned char ring[kStages][kStageBytes];
-  alignas(128) unsigned char enc[kParts][kTile * kXyzPad * 2];   // canonical [k8][row][8] hi (, lo)
+  static constexpr uint32_t kStageBytes = kStepBytes * (kKc / 16) * kParts;   // one full chunk
+  // what is left of the 227 KB after the activation buffers
+  static constexpr int kStages = kSplit ? 2 : 6;
+  alignas(128) unsigned char ring[kStages][kStageBytes];
+  alignas(128) unsigned char hid[kParts][kTile * kWidth * 2];    // canonical [k8][row][8] hi (, lo)
+  alignas(128) unsigned char enc[kParts][kTile * kXyzPad * 2];
   alignas(128) unsigned char dir[kParts][kTile * kDirPad * 2];
   alignas(16) float cst[kConstFloats];
-  float sigp[4][kTile];           // sigma head partial sums per 32-column group; [0] ends up holding sigma
-  // rgb head partial sums [4][3][kTile].  The split modes have no room for them and alias dir[0] (idle by then); the
-  // single-product mode has, which lets the encoder warps write the next dir embedding without waiting for rgb_done
-  float rgbp_own[kSplit ? 1 : 12 * kTile];
-  // training forward: per-warp 32 x 16 transposition tiles (row stride 20 words: conflict-free 128-bit
-  // accesses) so the activations leave as 64 contiguous bytes per 4 lanes instead of 16 bytes per lane
-  // at a 1 KB stride -- 8 lines per store instruction instead of 32
-  alignas(16) float store_tile[kTrain == 1 ? kEpiWarps : 1][kTrain == 1 ? 32 : 1][20];
-  uint64_t full[16], empty[16];
-  // (the rgb head's partial sums alias dir[0], idle by then: float [4][3][kTile])
-  uint64_t d_full[2], a_ready[4], a_free, enc_ready, dir_ready, d_drained;
-  uint64_t enc_free, dir_free;    // MMA -> encoder warps: the last MMA reading enc / dir of this slot has retired
-  uint64_t rgb_done;              // epilogue -> encoder warps: the rgb partial sums parked in dir[0] have been consumed
-  uint64_t d_full_dir;            // single-product mode: the direction layer's own "accumulator full" (without the d_drained
-                                  // hand-shake d_full[0] would see two completions -- the direction layer and the next
-                                  // layer 1 -- that no consumer observation separates)
-  uint32_t tmem_base;
+  uint64_t full[kStages], empty[kStages];
 };
 
 struct TcParams {
@@ -500,88 +383,60 @@ struct TcParams {
   unsigned char* a_g;      // (Ppad,128)
   uint32_t* a_mask;        // (8, 8, Ppad)
   long long ppad;
-  int debug;   // timing experiments only (SNB_TC_DEBUG): 2 = epilogue skips math, 4 = no MMAs
 };
-
-// ---- debug trace (SNB_TC_DEBUG & 8): clock64 stamps of one slot of cluster 0's leader CTA
-constexpr int kTraceLen = 2048;
-__device__ long long g_trace[kTraceLen];
-__device__ __forceinline__ void trace(bool on, int idx) { if (on && idx < kTraceLen) g_trace[idx] = clock64(); }
-
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 512;" ::: "memory"); }
 
 // canonical (SWIZZLE_NONE, K-major) byte offset of element (row, k) in a [k8][128 rows][8] block
 __device__ __forceinline__ uint32_t canon_off(int row, int k) { return (uint32_t)(k >> 3) * (kTile * 16) + row * 16 + (k & 7) * 2; }
 
-template <bool kBf16, bool kSplit, bool kEmbedded, int kCg, int kTrain = 0>
+// kTrain: 0 = inference, 1 = training forward keeping fp32 row-major activations (snb_field_forward_train),
+//         2 = training forward keeping fp16 activations in the T32 layout + ReLU mask words (act16.cuh)
+template <bool kBf16, bool kSplit, bool kEmbedded, int kTrain = 0>
 __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
   static_assert(!(kTrain != 0 && kEmbedded), "the training forward is the fused (rays, z) entry only");
-  using Smem = TcSmem<kSplit, kCg, kTrain>;
-  using G = Geo<kCg>;
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  Smem& s = *reinterpret_cast<Smem*>(smem_raw);
+  using Smem = TcSmem<kSplit>;
+  extern __shared__ unsigned char smem_raw[];
+  Smem& s = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr ConstLayout CL = make_const_layout();
-  constexpr uint32_t kStageBytes = Smem::kStageBytes;
   constexpr int kStages = Smem::kStages;
   constexpr int kParts = Smem::kParts;
-  static_assert(kStages <= 16, "barrier arrays");
-  const ChunkTable& tab = chunk_table<kCg>();
+  const ChunkTable& tab = c_chunks;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const PackedHeader* hdr = reinterpret_cast<const PackedHeader*>(p.image);
   const int new_activation = hdr->new_activation;
   const float* g_cst = reinterpret_cast<const float*>(p.image + sizeof(PackedHeader));
   const unsigned char* g_chunks = p.image + sizeof(PackedHeader) + kConstBytes;
-  const uint32_t cta_rank = kCg == 2 ? cluster_ctarank() : 0;
-  const bool leader = cta_rank == 0;
-  // tile slots: group g (a CTA or a CTA pair) handles tile (g + i * n_groups) * kCg + rank.  Every
-  // CTA of a group runs the same number of slots; slots past the end compute on zeros, store nothing.
   const long long ntiles = (p.n_points + kTile - 1) / kTile;
-  const long long n_groups = gridDim.x / kCg, group = blockIdx.x / kCg;
-  const long long n_slots = ((ntiles + kCg - 1) / kCg + n_groups - 1) / n_groups;
-  const int n_layers_epi = 8;   // trunk layers with a TMEM->TMEM epilogue (the bottleneck is folded away)
   const int n_chunks = p.sigma_only ? tab.n_sigma_only : tab.n_total;
-  // Deferred direction-layer epilogue (round 2, single-product mode).  The 128 softplus + rgb head of a tile are
-  // MUFU-bound (~2.8k cycles for the 16 epilogue warps) and used to run between the direction layer and the NEXT tile's
-  // layer-1 epilogue: the tensor pipe idled ~2.9k of a 26k-cycle slot at every slot boundary
-  // (profiles/r02b_trace_bf16_before_deferral.txt, chunk 2).  The single-product mode never uses the A-lo columns
-  // [384,512) of TMEM, so there the direction layer accumulates into THEM and the result simply stays: no drain, no
-  // d_drained hand-shake, the next tile's layer 1 starts at once, and the epilogue warps work the pre-activations off in
-  // four 8-column pieces (one tcgen05.ld each) in the windows where they wait for the next accumulator anyway -- after
-  // the second epilogue half of layers 1..4 of the next slot (slot 24.4k cycles, r02b_trace_bf16_deferred_dir_epilogue.txt).
-  // The split modes keep the in-place epilogue: TMEM is exactly full there, and a variant that parked the drained values
-  // in local memory shortened the slot by 4 % in cycles and not at all in time -- that kernel runs at the 1 kW power cap
-  // and the clock gave the cycles back (profiles/r02b_field_variants_ab.txt, r02b_trace_f16x3_deferred_experiment.txt).
-  constexpr bool kDirTmem = !kSplit && kTrain != 1;      // (the legacy fp32-storage training forward keeps the old order)
-  constexpr int kDirPieces = kDirTmem ? 4 : 1;
 
-  // ---------------- one-time setup
   for (int i = tid; i < kConstFloats; i += kThreads) s.cst[i] = g_cst[i];
   if (tid == 0) {
-    // full: this CTA's loader (+ the peer's relay, at the leader of a pair); a_ready / enc_ready live
-    // at the leader and count the epilogue threads of every CTA of the group
-    for (int i = 0; i < kStages; ++i) { mbar_init(&s.full[i], (kCg == 2 && leader) ? 2 : 1); mbar_init(&s.empty[i], 1); }
-    mbar_init(&s.d_full[0], 1); mbar_init(&s.d_full[1], 1); mbar_init(&s.a_free, 1);
-    for (int i = 0; i < 4; ++i) mbar_init(&s.a_ready[i], kEpiWarps * 16 * kCg);   // the two warps-of-four that own the quarter
-    mbar_init(&s.enc_ready, kEncWarps * 32 * kCg);
-    mbar_init(&s.dir_ready, kEncWarps * 32 * kCg);
-    mbar_init(&s.d_drained, kEpiWarps * 32 * kCg);
-    mbar_init(&s.enc_free, 1);
-    mbar_init(&s.dir_free, 1);
-    mbar_init(&s.rgb_done, kEpiWarps);
-    mbar_init(&s.d_full_dir, 1);
+    for (int i = 0; i < kStages; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], kWgs * 4); }
     fence_mbar_init();
   }
-  if (warp == kMmaWarp) { if (kCg == 2) tmem_alloc_pair(&s.tmem_base); else tmem_alloc<512>(&s.tmem_base); }
-  tc_fence_before();
   __syncthreads();
-  if (kCg == 2) cluster_sync_all();   // the peer's barriers exist before anyone signals them
-  tc_fence_after();
-  const uint32_t tbase = s.tmem_base;
 
-  // ---- helpers shared by the encoder and the epilogue warps
-  auto tile_of = [&](long long slot) { return (group + slot * n_groups) * kCg + cta_rank; };
-  // hand-off to the MMA issuer, which lives in the leader CTA
-  auto signal = [&](uint64_t* bar) { if (kCg == 2 && !leader) mbar_arrive_remote(bar, 0); else mbar_arrive(bar); };
+  // ---- weight stream: thread 0 keeps the ring kStages chunks ahead of consumption; a stage is refilled once
+  // all eight warps have released it
+  const long long my_tiles = ntiles > (long long)blockIdx.x ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+  const long long n_loads = my_tiles * n_chunks;
+  long long next_load = 0;
+  auto produce = [&](long long upto) {
+    for (; next_load < n_loads && next_load < upto; ++next_load) {
+      const uint32_t st = (uint32_t)(next_load % kStages), ph = (uint32_t)(next_load / kStages) & 1;
+      mbar_wait(&s.empty[st], ph ^ 1);
+      const Chunk c = tab.c[next_load % n_chunks];
+      const uint32_t bytes = kStepBytes * kParts * c.steps;
+      mbar_arrive_expect_tx(&s.full[st], bytes);
+      bulk_g2s(s.ring[st], g_chunks + (size_t)c.off * (kStepBytes * kParts), bytes, &s.full[st]);
+    }
+  };
+  if (tid == 0) produce(kStages);
+
+  // ======================= warpgroups =======================
+  const int wgi = warp >> 2, wq = warp & 3, tq = lane & 3;
+  const int r0 = wgi * 64 + wq * 16 + (lane >> 2);   // tile rows of this thread's accumulator fragments: r0, r0 + 8
+  auto wg_sync = [&]() { named_bar_sync(1 + wgi, 128); };
+
   // 16-bit storage: 8 consecutive features of one point -> one 16-byte cell of a T32 tensor
   auto store_cell16 = [&](unsigned char* base, long long pt, int f8, int F, const float (&v)[8]) {
     if (pt >= p.ppad) return;
@@ -600,629 +455,282 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
     *reinterpret_cast<uint4*>(hi_base + off) = make_uint4(h[0], h[1], h[2], h[3]);
     if (kSplit) *reinterpret_cast<uint4*>(lo_base + off) = make_uint4(l[0], l[1], l[2], l[3]);
   };
-  // 8 consecutive channels [c_lo, c_lo+8) of Embedding(3, L)(x): [x(3), sin(2^0 x)(3), cos(2^0 x)(3),
-  // sin(2^1 x)(3), ...] (nerf.py:36-41), one sincos per (frequency, coordinate) that the window touches
-  auto embed8 = [&](const float (&x)[3], int c_lo, int n_ch, int n_freqs, float (&v)[8]) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = (c_lo + j < 3) ? x[(c_lo + j) % 3] : 0.f;   // identity / zero pad
-    for (int f = 0; f < n_freqs; ++f) {
-      const int base = 3 + 6 * f;
-      if (base + 6 <= c_lo || base >= c_lo + 8) continue;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const int js = base + c - c_lo, jc = js + 3;
-        if ((js >= 0 && js < 8) || (jc >= 0 && jc < 8)) {
-          float sn, cs;
-          if (kSplit) sincosf(x[c] * (float)(1 << f), &sn, &cs);
-          else sincos_fast(x[c] * (float)(1 << f), &sn, &cs);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {           // static indices keep v[] in registers
-            if (j == js) v[j] = sn;
-            if (j == jc && base + 3 + c < n_ch) v[j] = cs;
-          }
-        }
+  // positional encoding of tile row r: xyz (Embedding(3, 10) of o + d z) or dir (Embedding(3, 4) of d)
+  auto encode_row = [&](long long tile, int r, bool xyz) {
+    const long long pt = tile * kTile + r;
+    const bool live = pt < p.n_points;
+    float x[3] = {0.f, 0.f, 0.f};
+    const float* xr = nullptr;
+    if (kEmbedded) {
+      xr = p.x + pt * p.x_stride;
+    } else if (live) {
+      const long long ray = pt / p.n_samples;
+      const float4 q0 = *reinterpret_cast<const float4*>(p.rays + ray * 8);
+      const float4 q1 = *reinterpret_cast<const float4*>(p.rays + ray * 8 + 4);
+      if (xyz) {
+        const float zz = p.z[pt];
+        x[0] = __fadd_rn(q0.x, __fmul_rn(q0.w, zz));   // rendering.py:284-285 rounding
+        x[1] = __fadd_rn(q0.y, __fmul_rn(q1.x, zz));
+        x[2] = __fadd_rn(q0.z, __fmul_rn(q1.y, zz));
+      } else {
+        x[0] = q0.w; x[1] = q1.x; x[2] = q1.y;          // ray direction (not normalised, rendering.py:261)
       }
+    }
+    auto emit = [&](auto ktag, const float (&v8)[8]) {
+      constexpr int k8 = decltype(ktag)::value;
+      if (!kEmbedded) {
+        if (kTrain == 1 && live) {
+          float4* dst = reinterpret_cast<float4*>((xyz ? p.save_enc + pt * kXyzPad : p.save_dir + pt * kDirPad) + k8 * 8);
+          dst[0] = make_float4(v8[0], v8[1], v8[2], v8[3]); dst[1] = make_float4(v8[4], v8[5], v8[6], v8[7]);
+        }
+        if (kTrain == 2) store_cell16(xyz ? p.a_enc : p.a_dir, pt, k8, xyz ? kXyzPad : kDirPad, v8);
+      }
+      if (xyz) put8(s.enc[0], s.enc[kSplit ? 1 : 0], k8, r, v8);
+      else put8(s.dir[0], s.dir[kSplit ? 1 : 0], k8, r, v8);
+    };
+    auto encode_all = [&](auto ltag) {
+      constexpr int L = decltype(ltag)::value;            // 10 (xyz, 63 -> 64 channels) or 4 (dir, 27 -> 32)
+      constexpr int kCh = 3 * (2 * L + 1), kPad = (kCh + 7) / 8 * 8;
+      float v[kPad];
+#pragma unroll
+      for (int j = 0; j < kPad; ++j) v[j] = 0.f;
+      if (kEmbedded) {
+        const int nin = p.sigma_only ? kXyzCh : kXyzCh + kDirCh;
+#pragma unroll
+        for (int j = 0; j < kCh; ++j) {
+          const int col = L == SNB_XYZ_FREQS ? j : kXyzCh + j;
+          v[j] = (live && col < nin) ? xr[col] : 0.f;
+        }
+      } else {
+        v[0] = x[0]; v[1] = x[1]; v[2] = x[2];
+#pragma unroll
+        for (int f = 0; f < L; ++f)
+#pragma unroll
+          for (int c = 0; c < 3; ++c) {
+            float sn, cs;
+            if (kSplit) sincosf(x[c] * (float)(1 << f), &sn, &cs);
+            else sincos_fast(x[c] * (float)(1 << f), &sn, &cs);
+            v[3 + 6 * f + c] = sn;
+            v[3 + 6 * f + 3 + c] = cs;
+          }
+      }
+      static_for<kPad / 8>([&](auto ktag) {
+        constexpr int k8 = decltype(ktag)::value;
+        const float v8[8] = {v[8 * k8], v[8 * k8 + 1], v[8 * k8 + 2], v[8 * k8 + 3], v[8 * k8 + 4], v[8 * k8 + 5], v[8 * k8 + 6], v[8 * k8 + 7]};
+        emit(ktag, v8);
+      });
+    };
+    if (xyz) encode_all(std::integral_constant<int, SNB_XYZ_FREQS>{});
+    else encode_all(std::integral_constant<int, SNB_DIR_FREQS>{});
+  };
+
+  auto mma = [&](float (&d)[64], uint64_t a, uint64_t b, uint32_t accumulate) {
+    if (kBf16) wgmma_m64n128_bf16(d, a, b, accumulate);
+    else wgmma_m64n128_f16(d, a, b, accumulate);
+  };
+  // K16 step ks of the current chunk into accumulator d: hi*hi (+ lo*hi + hi*lo)
+  auto issue_step = [&](float (&d)[64], uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl, uint32_t accumulate) {
+    const uint64_t da_h = make_smem_desc(ah, kTile * 16, 128), db_h = make_smem_desc(bh, kNh * 16, 128);
+    mma(d, da_h, db_h, accumulate);
+    if (kSplit) {
+      mma(d, make_smem_desc(al, kTile * 16, 128), db_h, 1u);
+      mma(d, da_h, make_smem_desc(bl, kNh * 16, 128), 1u);
     }
   };
 
-  if (warp == kLoadWarp) {
-    // ======================= weight loader (one elected lane) =======================
-    // streams this CTA's share of every chunk, in schedule order, through the ring
-    if (elect_one()) {
-      uint32_t it = 0;
-      for (long long slot = 0; slot < n_slots; ++slot) {
-        for (int ci = 0; ci < n_chunks; ++ci, ++it) {
-          const uint32_t st = it % kStages, ph = (it / kStages) & 1;
-          mbar_wait(&s.empty[st], ph ^ 1);
-          const Chunk c = tab.c[ci];
-          const uint32_t share = G::kStepBytes * kParts * c.steps;      // this CTA's bytes of the chunk
-          const unsigned char* src = g_chunks + (size_t)c.off * (G::kStepBytes * kParts * kCg) + (size_t)cta_rank * share;
-          mbar_arrive_expect_tx(&s.full[st], share);
-          for (uint32_t o = 0; o < share; o += 16384)
-            bulk_g2s(s.ring[st] + o, src + o, share - o < 16384 ? share - o : 16384, &s.full[st]);
-        }
-      }
-    }
-  } else if (warp == kMmaWarp && !leader) {
-    // ======================= relay (odd CTA of a pair) =======================
-    // tells the leader when this CTA's share of a chunk has landed
-    if (elect_one()) {
-      uint32_t it = 0;
-      for (long long slot = 0; slot < n_slots; ++slot) {
-        for (int ci = 0; ci < n_chunks; ++ci, ++it) {
-          const uint32_t st = it % kStages, ph = (it / kStages) & 1;
-          mbar_wait(&s.full[st], ph);
-          mbar_arrive_remote(&s.full[st], 0);
-        }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    // ======================= MMA issuer (leader CTA) =======================
-    // One elected lane runs the whole role.  The chunk schedule is unrolled at compile time
-    // (static_for over the constexpr table): every wait, operand offset, accumulate flag and
-    // commit of a chunk is an immediate, so a chunk costs a few dozen instructions besides its
-    // MMAs.  (Measured: the table-driven loop spent ~200 instructions / ~1000 cycles per chunk,
-    // more than the 515 cycles the tensor pipe needs for a bf16 chunk -- the issuer, not the
-    // pipe, set the pace; profiles/r01_timing_experiments.txt v11.)
-    if (elect_one()) {
-      constexpr ChunkTable T = make_chunk_table<G::kKc>();
-      const uint32_t idesc = make_idesc(kBf16 ? kFmtBF16 : kFmtF16, kTile * kCg, kNh);
-      const uint32_t enc_hi = smem_u32(s.enc[0]), dir_hi = smem_u32(s.dir[0]);
-      const uint32_t enc_lo = smem_u32(s.enc[kSplit ? 1 : 0]), dir_lo = smem_u32(s.dir[kSplit ? 1 : 0]);
-      // descriptors as (lo, hi) words: only the 14-bit start-address field in the low word moves
-      const uint64_t desc_b0 = make_smem_desc(0, G::kRowsB * 16, 128);
-      const uint64_t desc_a0 = make_smem_desc(0, kTile * 16, 128);
-      const uint32_t bd_hi32 = (uint32_t)(desc_b0 >> 32), ad_hi32 = (uint32_t)(desc_a0 >> 32);
-      const uint32_t b_ring0 = (uint32_t)desc_b0 + (smem_u32(s.ring[0]) >> 4);
-      const uint32_t a_enc_hi = (uint32_t)desc_a0 + (enc_hi >> 4), a_enc_lo = (uint32_t)desc_a0 + (enc_lo >> 4);
-      const uint32_t a_dir_hi = (uint32_t)desc_a0 + (dir_hi >> 4), a_dir_lo = (uint32_t)desc_a0 + (dir_lo >> 4);
-      constexpr uint32_t kStepB = (2 * G::kRowsB * 16) >> 4;     // one K16 step inside a chunk, in 16-B units
-      constexpr uint32_t kStepA = (2 * kTile * 16) >> 4;
-      auto commit = [&](uint64_t* bar) { if (kCg == 2) mma2_commit(bar); else mma_commit(bar); };
-      const bool do_mma = !(p.debug & 4);
-      uint32_t st = 0, ph_full = 0;            // ring position: stage and the parity of its `full` barrier
-      for (long long slot = 0; slot < n_slots; ++slot) {
-        const uint32_t slot_par = (uint32_t)slot & 1;    // enc_ready / dir_ready / d_drained complete once per slot
-        const bool tr = (p.debug & 8) && blockIdx.x == 0 && slot == 3;
-        static_for<T.n_total>([&](auto tag) {
-          constexpr int CI = decltype(tag)::value;
-          constexpr Chunk c = T.c[CI];
-          if (CI >= T.n_sigma_only && p.sigma_only) return;
-          trace(tr, CI * 4 + 0);
-          // a_ready[q] completes 8 times per slot (static_assert below): the parity of each wait is static
-          auto wait_code = [&](auto code_tag, auto stage_tag) {
-            constexpr int w = decltype(code_tag)::value;
-            if (w == WAIT_ENC) mbar_wait(&s.enc_ready, slot_par);
-            else if (w == WAIT_DIR) mbar_wait(&s.dir_ready, slot_par);
-            else if (w >= WAIT_A0) mbar_wait(&s.a_ready[w - WAIT_A0], prior_waits(T, CI, w, decltype(stage_tag)::value) & 1);
-          };
-          wait_code(std::integral_constant<int, c.wait>{}, std::integral_constant<int, 0>{});
-          wait_code(std::integral_constant<int, c.wait2>{}, std::integral_constant<int, 1>{});
-          trace(tr, CI * 4 + 1);
-          mbar_wait(&s.full[st], ph_full);
-          tc_fence_after();
-          trace(tr, CI * 4 + 2);
-          const uint32_t d = tbase + (c.layer == 9 ? (kDirTmem ? kColAlo : kColD) : kColD + c.half * kNh);
-          const uint32_t bh = b_ring0 + st * (kStageBytes >> 4);           // W_hi block
-          const uint32_t bl = bh + ((G::kStepBytes * c.steps) >> 4);        // W_lo block
-          // K16 steps [kLo, kHi) of this chunk
-          auto issue_range = [&](auto lo_tag, auto hi_tag) {
-            constexpr int kLo = decltype(lo_tag)::value, kHi = decltype(hi_tag)::value;
-            if (c.src == SRC_HID) {
-              const uint32_t a_hi = tbase + kColAhi + (uint32_t)c.a16 * 8;
-              const uint32_t a_lo = tbase + kColAlo + (uint32_t)c.a16 * 8;
+  float acc0[64], acc1[64];
+  float sig[2] = {0.f, 0.f};     // sigma of rows r0, r0 + 8 (layer 8's epilogue -> the direction layer's)
+  uint32_t it = 0;
+
+  // trunk epilogue of layer l (0..7): bias, ReLU, hi/lo split -> the next layer's A operand in shared memory
+  auto trunk_epilogue = [&](int l, long long pt0) {
+    const float* bias = s.cst + CL.b[l];
+    unsigned char* hb = kTrain == 2 ? p.a_h + (size_t)l * (size_t)p.ppad * (kWidth * 2) : nullptr;
+    const bool sigma_layer = l == 7;
+    if (sigma_layer) { sig[0] = 0.f; sig[1] = 0.f; }
 #pragma unroll
-              for (int ks = kLo; ks < kHi; ++ks) {
-                const uint32_t acc = (ks == 0 && c.first) ? 0u : 1u;
-                if (kCg == 2) {
-                  mma2_ts_lohi(d, a_hi + ks * 8, bh + ks * kStepB, bd_hi32, idesc, acc);
-                  if (kSplit) {
-                    mma2_ts_lohi(d, a_lo + ks * 8, bh + ks * kStepB, bd_hi32, idesc, 1);
-                    mma2_ts_lohi(d, a_hi + ks * 8, bl + ks * kStepB, bd_hi32, idesc, 1);
-                  }
-                } else {
-                  const uint64_t b1 = ((uint64_t)bd_hi32 << 32) | (bh + ks * kStepB), b2 = ((uint64_t)bd_hi32 << 32) | (bl + ks * kStepB);
-                  mma_ts(d, a_hi + ks * 8, b1, idesc, acc);
-                  if (kSplit) { mma_ts(d, a_lo + ks * 8, b1, idesc, 1); mma_ts(d, a_hi + ks * 8, b2, idesc, 1); }
-                }
-              }
-            } else {
-              constexpr uint32_t a_off = ((uint32_t)c.a16 * 2 * (kTile * 16)) >> 4;
-              const uint32_t ah = (c.src == SRC_ENC ? a_enc_hi : a_dir_hi) + a_off;
-              const uint32_t al = (c.src == SRC_ENC ? a_enc_lo : a_dir_lo) + a_off;
+    for (int h = 0; h < 2; ++h) {
+      float (&d)[64] = h ? acc1 : acc0;
+      uint32_t mw[2] = {0u, 0u};
 #pragma unroll
-              for (int ks = kLo; ks < kHi; ++ks) {
-                const uint32_t acc = (ks == 0 && c.first) ? 0u : 1u;
-                if (kCg == 2) {
-                  mma2_ss_lohi(d, ah + ks * kStepA, ad_hi32, bh + ks * kStepB, bd_hi32, idesc, acc);
-                  if (kSplit) {
-                    mma2_ss_lohi(d, al + ks * kStepA, ad_hi32, bh + ks * kStepB, bd_hi32, idesc, 1);
-                    mma2_ss_lohi(d, ah + ks * kStepA, ad_hi32, bl + ks * kStepB, bd_hi32, idesc, 1);
-                  }
-                } else {
-                  const uint64_t a1 = ((uint64_t)ad_hi32 << 32) | (ah + ks * kStepA), a2 = ((uint64_t)ad_hi32 << 32) | (al + ks * kStepA);
-                  const uint64_t b1 = ((uint64_t)bd_hi32 << 32) | (bh + ks * kStepB), b2 = ((uint64_t)bd_hi32 << 32) | (bl + ks * kStepB);
-                  mma_ss(d, a1, b1, idesc, acc);
-                  if (kSplit) { mma_ss(d, a2, b1, idesc, 1); mma_ss(d, a1, b2, idesc, 1); }
-                }
-              }
-            }
-          };
-          using I0 = std::integral_constant<int, 0>;
-          using IM = std::integral_constant<int, c.mid>;
-          using IS = std::integral_constant<int, c.steps>;
-          if (do_mma) issue_range(I0{}, IM{});
-          trace(tr, 512 + CI * 4 + 0);
-          if (c.mid < c.steps) {            // the chunk spans two K quarters: the second arrives later
-            wait_code(std::integral_constant<int, c.wait_mid>{}, std::integral_constant<int, 2>{});
-            tc_fence_after();
-            if (do_mma) issue_range(IM{}, IS{});
-            trace(tr, 512 + CI * 4 + 1);
-          }
-          commit(&s.empty[st]);        // ring slot free (in both CTAs of a pair) once these MMAs retire
-          trace(tr, 512 + CI * 4 + 2);
-          if (c.commit & COMMIT_AFREE) commit(&s.a_free);
-          if (c.commit & COMMIT_D0) commit((c.layer == 9 && kDirTmem) ? &s.d_full_dir : &s.d_full[0]);
-          if (c.commit & COMMIT_D1) commit(&s.d_full[1]);
-          if (c.src == SRC_ENC && c.layer == 4 && c.half == 1) commit(&s.enc_free);   // last reader of enc in this slot
-          if (c.src == SRC_DIR) commit(&s.dir_free);
-          trace(tr, 512 + CI * 4 + 3);
-          if (++st == kStages) { st = 0; ph_full ^= 1; }
-          trace(tr, CI * 4 + 3);
-        });
-        if (p.sigma_only) {
-          // layer 8's epilogue arrives on a_ready[0..3] with nobody waiting: consume the phases
+      for (int j = 0; j < 16; ++j) {
+        const int col = h * kNh + 8 * j + 2 * tq;
+        const float2 bb = *reinterpret_cast<const float2*>(bias + col);
 #pragma unroll
-          for (int q = 0; q < 4; ++q) mbar_wait(&s.a_ready[q], prior_waits(T, T.n_sigma_only, WAIT_A0 + q, 0) & 1);
-        } else if (!kDirTmem) {
-          // the next slot's layer 1 overwrites D[0,128): wait until the dir-layer epilogue has read it
-          // (kDirTmem: the direction layer has its own accumulator; its next overwrite is ordered behind the
-          // a_ready waits of the next slot's layer 8, which every epilogue thread signals after its last piece)
-          mbar_wait(&s.d_drained, slot_par);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp >= kEncWarp0) {
-    // ======================= encoder warps: positional encodings of the NEXT slot =======================
-    // 64 threads, two tile rows each.  In round 1 the epilogue warps did this in their idle windows; in the
-    // single-product bf16 mode (512-cycle MMA phases) those windows do not exist and the encodings -- global loads of
-    // the ray and depth, a 64-bit division, 30 sin/cos pairs -- sat on the layer-to-layer critical path: ~8k of a
-    // 30k-cycle slot (profiles/r02_trace_bf16_fast_trig.txt).  Here they run beside everything else: xyz for slot s+1
-    // as soon as the skip layer of slot s has consumed enc (enc_free), dir as soon as the direction layer has (dir_free).
-    const int e = (warp - kEncWarp0) * 32 + lane;
-    auto encode_rows = [&](long long slot, bool xyz) {
-#pragma unroll 1
-      for (int rr = 0; rr < kTile / (kEncWarps * 32); ++rr) {
-        const int r = e + rr * (kEncWarps * 32);
-        const long long pt = tile_of(slot) * kTile + r;
-        const bool live = pt < p.n_points;
-        float x[3] = {0.f, 0.f, 0.f};
-        const float* xr = nullptr;
-        if (kEmbedded) {
-          xr = p.x + pt * p.x_stride;
-        } else if (live) {
-          const long long ray = pt / p.n_samples;
-          const float4 r0 = *reinterpret_cast<const float4*>(p.rays + ray * 8);
-          const float4 r1 = *reinterpret_cast<const float4*>(p.rays + ray * 8 + 4);
-          if (xyz) {
-            const float zz = p.z[pt];
-            x[0] = __fadd_rn(r0.x, __fmul_rn(r0.w, zz));   // rendering.py:284-285 rounding
-            x[1] = __fadd_rn(r0.y, __fmul_rn(r1.x, zz));
-            x[2] = __fadd_rn(r0.z, __fmul_rn(r1.y, zz));
+        for (int rr = 0; rr < 2; ++rr) {
+          const int row = r0 + 8 * rr;
+          const long long pt = pt0 + 8 * rr;
+          float x0 = d[4 * j + 2 * rr] + bb.x, x1 = d[4 * j + 2 * rr + 1] + bb.y;
+          uint32_t hi, lo;
+          if (kTrain == 0 && !sigma_layer) {
+            // nobody needs the fp32 post-activation value: ReLU and the fp16 range guard ride on the converts
+            split_pair_relu<kBf16, kSplit>(x0, x1, hi, lo);
           } else {
-            x[0] = r0.w; x[1] = r1.x; x[2] = r1.y;          // ray direction (not normalised, rendering.py:261)
+            x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f);
+            if (sigma_layer) {
+              const float2 ww = *reinterpret_cast<const float2*>(s.cst + CL.sigma_w + col);
+              sig[rr] = fmaf(x0, ww.x, sig[rr]); sig[rr] = fmaf(x1, ww.y, sig[rr]);
+            }
+            split_pair<kBf16, kSplit, true>(x0, x1, hi, lo);
+            if (kTrain == 1 && pt < p.n_points)
+              *reinterpret_cast<float2*>(p.save_h + ((size_t)l * p.n_points + pt) * kWidth + col) = make_float2(x0, x1);
+            if (kTrain == 2) {
+              // fp16 modes: the hi word of the split IS rn_fp16(value) (saturated); bf16 modes convert separately
+              const uint32_t h16 = kBf16 ? pack_half2_sat(x0, x1) : hi;
+              if (pt < p.ppad)
+                *reinterpret_cast<uint32_t*>(hb + a16_cell(pt, col >> 3, kWidth) + (col & 7) * 2) = pt < p.n_points ? h16 : 0u;
+              mw[rr] |= ((x0 > 0.f ? 1u : 0u) << (col & 31)) | ((x1 > 0.f ? 1u : 0u) << ((col & 31) + 1));
+            }
+          }
+          const uint32_t off = canon_off(row, col);
+          *reinterpret_cast<uint32_t*>(s.hid[0] + off) = hi;
+          if (kSplit) *reinterpret_cast<uint32_t*>(s.hid[kSplit ? 1 : 0] + off) = lo;
+        }
+        if (kTrain == 2 && (j & 3) == 3) {
+          // a 32-column group is complete: the quad's four threads hold its 32 ReLU bits of each row
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            uint32_t w = mw[rr];
+            w |= __shfl_xor_sync(0xffffffffu, w, 1);
+            w |= __shfl_xor_sync(0xffffffffu, w, 2);
+            const long long pt = pt0 + 8 * rr;
+            if (tq == 0 && pt < p.ppad) p.a_mask[a16_mask_index(l, col >> 5, pt, p.ppad)] = pt < p.n_points ? w : 0u;
+            mw[rr] = 0u;
           }
         }
-        // all channels of the row in registers, one sin / cos pair per (frequency, coordinate): static indices only
-        auto emit = [&](auto ktag, const float (&v8)[8]) {
-          constexpr int k8 = decltype(ktag)::value;
-          if (!kEmbedded) {
-            if (kTrain == 1 && live) {
-              float4* dst = reinterpret_cast<float4*>((xyz ? p.save_enc + pt * kXyzPad : p.save_dir + pt * kDirPad) + k8 * 8);
-              dst[0] = make_float4(v8[0], v8[1], v8[2], v8[3]); dst[1] = make_float4(v8[4], v8[5], v8[6], v8[7]);
-            }
-            if (kTrain == 2) store_cell16(xyz ? p.a_enc : p.a_dir, pt, k8, xyz ? kXyzPad : kDirPad, v8);
-          }
-          if (xyz) put8(s.enc[0], s.enc[kSplit ? 1 : 0], k8, r, v8);
-          else put8(s.dir[0], s.dir[kSplit ? 1 : 0], k8, r, v8);
-        };
-        auto encode_all = [&](auto ltag) {
-          constexpr int L = decltype(ltag)::value;            // 10 (xyz, 63 -> 64 channels) or 4 (dir, 27 -> 32)
-          constexpr int kCh = 3 * (2 * L + 1), kPad = (kCh + 7) / 8 * 8;
-          float v[kPad];
-#pragma unroll
-          for (int j = 0; j < kPad; ++j) v[j] = 0.f;
-          if (kEmbedded) {
-            const int nin = p.sigma_only ? kXyzCh : kXyzCh + kDirCh;
-#pragma unroll
-            for (int j = 0; j < kCh; ++j) {
-              const int col = L == SNB_XYZ_FREQS ? j : kXyzCh + j;
-              v[j] = (live && col < nin) ? xr[col] : 0.f;
-            }
-          } else {
-            v[0] = x[0]; v[1] = x[1]; v[2] = x[2];
-#pragma unroll
-            for (int f = 0; f < L; ++f)
-#pragma unroll
-              for (int c = 0; c < 3; ++c) {
-                float sn, cs;
-                if (kSplit) sincosf(x[c] * (float)(1 << f), &sn, &cs);
-                else sincos_fast(x[c] * (float)(1 << f), &sn, &cs);
-                v[3 + 6 * f + c] = sn;
-                v[3 + 6 * f + 3 + c] = cs;
-              }
-          }
-          static_for<kPad / 8>([&](auto ktag) {
-            constexpr int k8 = decltype(ktag)::value;
-            const float v8[8] = {v[8 * k8], v[8 * k8 + 1], v[8 * k8 + 2], v[8 * k8 + 3], v[8 * k8 + 4], v[8 * k8 + 5], v[8 * k8 + 6], v[8 * k8 + 7]};
-            emit(ktag, v8);
-          });
-        };
-        if (xyz) encode_all(std::integral_constant<int, SNB_XYZ_FREQS>{});
-        else encode_all(std::integral_constant<int, SNB_DIR_FREQS>{});
-      }
-      fence_proxy_async_smem();     // generic-proxy smem writes -> visible to tcgen05.mma
-      signal(xyz ? &s.enc_ready : &s.dir_ready);
-    };
-    if (n_slots > 0) {
-      encode_rows(0, true);
-      if (!p.sigma_only) encode_rows(0, false);
-    }
-    for (long long slot = 0; slot + 1 < n_slots; ++slot) {
-      mbar_wait(&s.enc_free, (uint32_t)slot & 1);
-      encode_rows(slot + 1, true);
-      if (!p.sigma_only) {
-        mbar_wait(&s.dir_free, (uint32_t)slot & 1);
-        if (kSplit) mbar_wait(&s.rgb_done, (uint32_t)slot & 1);    // the rgb partial sums alias dir[0] there
-        encode_rows(slot + 1, false);
       }
     }
-  } else {
-    // ======================= prologue / epilogue warps =======================
-    const int quad = warp & 3, ch = warp >> 2;       // TMEM lane quadrant, 32-column group (0..3) of a 128-column half
-    const int row = quad * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(quad * 32) << 16;
-    uint32_t ph_d = 0, ph_free = 0;       // ph_d: bit h = parity of d_full[h]
-    // training forward: 16 consecutive columns of this warp's 32 rows -> global, through the warp's tile.
-    // `x4[k]` = this thread's row, columns [4k, 4k+4); dst_block = address of (first row of the block, first column)
-    auto store_block16 = [&](const float4 (&x4)[4], float* dst_block, long long ld, long long pt_block0) {
-      float (*tile)[20] = s.store_tile[kTrain == 1 ? warp : 0];
+    if (sigma_layer) {
+      // sigma head (nerf.py:136): the quad's four threads hold the row's columns
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        float v = sig[rr];
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        sig[rr] = v + s.cst[CL.sigma_b];
+        const long long pt = pt0 + 8 * rr;
+        if (p.sigma_only && tq == 0 && pt < p.n_points) p.out[pt] = sig[rr];
+      }
+    }
+    fence_proxy_async_smem();     // generic-proxy smem writes -> visible to the next layer's wgmmas
+    wg_sync();
+  };
+
+  // direction layer: shifted softplus / ReLU, rgb head (nerf.py:142-146), the [r, g, b, sigma] rows
+  auto dir_epilogue = [&](long long pt0) {
+    const float sh = new_activation ? 1.0f : 0.0f;   // shifted softplus: fold the -1 into the bias
+    float a[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int col = 8 * j + 2 * tq;
+      const float2 bb = *reinterpret_cast<const float2*>(s.cst + CL.b[9] + col);
+      const float2 w0 = *reinterpret_cast<const float2*>(s.cst + CL.rgb_w + col);
+      const float2 w1 = *reinterpret_cast<const float2*>(s.cst + CL.rgb_w + kHalf + col);
+      const float2 w2 = *reinterpret_cast<const float2*>(s.cst + CL.rgb_w + 2 * kHalf + col);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const long long pt = pt0 + 8 * rr;
+        float x0 = acc0[4 * j + 2 * rr] + (bb.x - sh), x1 = acc0[4 * j + 2 * rr + 1] + (bb.y - sh);
+        if (new_activation) { x0 = softplus_fast(x0); x1 = softplus_fast(x1); }
+        else { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        if (kTrain == 1 && pt < p.n_points) *reinterpret_cast<float2*>(p.save_g + pt * kHalf + col) = make_float2(x0, x1);
+        if (kTrain == 2 && pt < p.ppad)
+          *reinterpret_cast<uint32_t*>(p.a_g + a16_cell(pt, col >> 3, kHalf) + (col & 7) * 2) =
+              pt < p.n_points ? pack_half2_sat(x0, x1) : 0u;
+        a[rr][0] = fmaf(x1, w0.y, fmaf(x0, w0.x, a[rr][0]));
+        a[rr][1] = fmaf(x1, w1.y, fmaf(x0, w1.x, a[rr][1]));
+        a[rr][2] = fmaf(x1, w2.y, fmaf(x0, w2.x, a[rr][2]));
+      }
+    }
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      float c[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        float v = a[rr][k];
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        v += s.cst[CL.rgb_b + k];
+        c[k] = new_activation ? widened_sigmoid_f(v) : sigmoid_f(v);
+      }
+      const long long pt = pt0 + 8 * rr;
+      if (tq == 0 && pt < p.n_points) reinterpret_cast<float4*>(p.out)[pt] = make_float4(c[0], c[1], c[2], sig[rr]);
+    }
+  };
+
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const long long pt0 = tile * kTile + r0;
+    // ---- encodings of this warpgroup's 64 rows: threads 0..63 xyz, 64..127 dir
+    {
+      const int e = tid & 127;
+      if (e < 64) encode_row(tile, wgi * 64 + e, true);
+      else if (!p.sigma_only) encode_row(tile, wgi * 64 + e - 64, false);
+      fence_proxy_async_smem();
+      wg_sync();
+    }
+    int pend = -1;    // ring stage whose wgmmas are committed but not yet released
+    for (int ci = 0; ci < n_chunks; ++ci, ++it) {
+      const Chunk c = tab.c[ci];
+      if (c.first && c.half == 0) {
+        // a new layer: the accumulators are overwritten (accumulate = 0); defining them here ends their
+        // live range at the previous epilogue
+#pragma unroll
+        for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+      }
+      const uint32_t st = it % kStages, ph = (it / kStages) & 1;
+      mbar_wait(&s.full[st], ph);
+      wgmma_fence();
+      const uint32_t bh = smem_u32(s.ring[st]), bl = bh + kStepBytes * c.steps;
+      const unsigned char* abuf = c.src == SRC_HID ? s.hid[0] : (c.src == SRC_ENC ? s.enc[0] : s.dir[0]);
+      const uint32_t part = c.src == SRC_HID ? (uint32_t)sizeof(s.hid[0]) : (c.src == SRC_ENC ? (uint32_t)sizeof(s.enc[0]) : (uint32_t)sizeof(s.dir[0]));
+      const uint32_t ah = smem_u32(abuf) + wgi * 64 * 16 + (uint32_t)c.a16 * 2 * (kTile * 16);
+#pragma unroll
+      for (int ks = 0; ks < kKc / 16; ++ks) {
+        if (ks < c.steps) {
+          const uint32_t accumulate = (ks == 0 && c.first) ? 0u : 1u;
+          const uint32_t a_k = ah + ks * 2 * (kTile * 16), b_k = ks * kStepBytes;
+          if (c.half == 0) issue_step(acc0, a_k, a_k + part, bh + b_k, bl + b_k, accumulate);
+          else issue_step(acc1, a_k, a_k + part, bh + b_k, bl + b_k, accumulate);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                                      // the previous chunk's wgmmas have retired
+      if (pend >= 0 && lane == 0) mbar_arrive(&s.empty[pend]);
+      pend = (int)st;
+      if (tid == 0) produce((long long)it + kStages);
       __syncwarp();
-#pragma unroll
-      for (int k = 0; k < 4; ++k) *reinterpret_cast<float4*>(&tile[lane][4 * k]) = x4[k];
-      __syncwarp();
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = (lane >> 2) + 8 * i, c = lane & 3;
-        if (pt_block0 + r < p.n_points)
-          *reinterpret_cast<float4*>(dst_block + r * ld + 4 * c) = *reinterpret_cast<const float4*>(&tile[r][4 * c]);
+      if (ci + 1 == n_chunks || tab.c[ci + 1].layer != c.layer) {
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&s.empty[pend]);
+        pend = -1;
+        if (c.layer == 9) dir_epilogue(pt0);
+        else trunk_epilogue(c.layer, pt0);
       }
-    };
-
-    // ---------------- direction-layer epilogue (shifted softplus / ReLU, rgb head), in pieces
-    constexpr int kJ4 = 8 / kDirPieces;          // groups of four columns per piece (this thread owns 32 columns)
-    const int cdir0 = ch * 32;
-    // rgb partial sums go through the dir-embedding buffer: its last readers (the dir-layer MMAs of the tile the sums
-    // belong to) have retired, and the encoder warps write the next dir embedding only after rgb_done
-    float* rgbp = kSplit ? reinterpret_cast<float*>(s.dir[0]) : s.rgbp_own;     // [4][3][kTile]
-    // piece `pc` of the tile whose row of this thread is point `dpt`; `vreg` = the 32 drained values (in-place epilogue)
-    auto dir_piece = [&](int pc, long long dpt, const uint32_t* vreg) {
-      const int col0 = cdir0 + pc * (4 * kJ4);
-      const float4* b4 = reinterpret_cast<const float4*>(s.cst + CL.b[9] + col0);
-      const float4* w0 = reinterpret_cast<const float4*>(s.cst + CL.rgb_w + col0);
-      const float4* w1 = reinterpret_cast<const float4*>(s.cst + CL.rgb_w + kHalf + col0);
-      const float4* w2 = reinterpret_cast<const float4*>(s.cst + CL.rgb_w + 2 * kHalf + col0);
-      float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-      if (pc > 0) { a0 = rgbp[(ch * 3 + 0) * kTile + row]; a1 = rgbp[(ch * 3 + 1) * kTile + row]; a2 = rgbp[(ch * 3 + 2) * kTile + row]; }
-      uint32_t t8[kDirTmem ? 8 : 1];
-      if constexpr (kDirTmem) {
-        static_assert(!kDirTmem || kJ4 == 2, "a piece is one 8-column tcgen05.ld");
-        tmem_ld8(tbase + lane_base + kColAlo + col0, t8);
-        tmem_wait_ld();
-      }
-      uint32_t g16[kTrain == 2 ? 2 * kJ4 : 1];   // this piece's direction-layer outputs as fp16 pairs
-      float4 keep[4];
-      const float sh = new_activation ? 1.0f : 0.0f;   // shifted softplus: fold the -1 into the bias
-#pragma unroll
-      for (int jj = 0; jj < kJ4; ++jj) {
-        const float4 bb = b4[jj], r0 = w0[jj], r1 = w1[jj], r2 = w2[jj];
-        float x[4];
-        if constexpr (kDirTmem) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) x[e] = __uint_as_float(t8[4 * jj + e]);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) x[e] = __uint_as_float(vreg[4 * jj + e]);
-        }
-        x[0] += bb.x - sh; x[1] += bb.y - sh; x[2] += bb.z - sh; x[3] += bb.w - sh;
-        if (new_activation) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) x[e] = softplus_fast(x[e]);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) x[e] = fmaxf(x[e], 0.f);
-        }
-        if (kTrain == 1) {
-          keep[jj & 3] = make_float4(x[0], x[1], x[2], x[3]);
-          if ((jj & 3) == 3) store_block16(keep, p.save_g + (dpt - lane) * kHalf + cdir0 + (jj >> 2) * 16, kHalf, dpt - lane);
-        }
-        if (kTrain == 2) { g16[2 * jj] = pack_half2_sat(x[0], x[1]); g16[2 * jj + 1] = pack_half2_sat(x[2], x[3]); }
-        a0 = fmaf(x[0], r0.x, a0); a0 = fmaf(x[1], r0.y, a0); a0 = fmaf(x[2], r0.z, a0); a0 = fmaf(x[3], r0.w, a0);
-        a1 = fmaf(x[0], r1.x, a1); a1 = fmaf(x[1], r1.y, a1); a1 = fmaf(x[2], r1.z, a1); a1 = fmaf(x[3], r1.w, a1);
-        a2 = fmaf(x[0], r2.x, a2); a2 = fmaf(x[1], r2.y, a2); a2 = fmaf(x[2], r2.z, a2); a2 = fmaf(x[3], r2.w, a2);
-      }
-      if (kTrain == 2 && dpt < p.ppad) {
-        const bool live = dpt < p.n_points;
-#pragma unroll
-        for (int c = 0; c < kJ4 / 2; ++c)
-          *reinterpret_cast<uint4*>(p.a_g + a16_cell(dpt, (col0 >> 3) + c, kHalf)) =
-              live ? make_uint4(g16[4 * c], g16[4 * c + 1], g16[4 * c + 2], g16[4 * c + 3]) : make_uint4(0u, 0u, 0u, 0u);
-      }
-      rgbp[(ch * 3 + 0) * kTile + row] = a0; rgbp[(ch * 3 + 1) * kTile + row] = a1; rgbp[(ch * 3 + 2) * kTile + row] = a2;
-    };
-    // rgb head (nerf.py:144) + the tile's [r, g, b, sigma] rows
-    auto dir_finish = [&](long long dpt) {
-      epi_bar_sync();
-      if (ch == 0 && dpt < p.n_points) {
-        float c[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          const float x = ((rgbp[k * kTile + row] + rgbp[(3 + k) * kTile + row]) +
-                           (rgbp[(6 + k) * kTile + row] + rgbp[(9 + k) * kTile + row])) + s.cst[CL.rgb_b + k];
-          c[k] = new_activation ? widened_sigmoid_f(x) : sigmoid_f(x);
-        }
-        reinterpret_cast<float4*>(p.out)[dpt] = make_float4(c[0], c[1], c[2], s.sigp[0][row]);
-      }
-      epi_bar_sync();
-      if (lane == 0) mbar_arrive(&s.rgb_done);
-    };
-    bool pending = false;      // the previous slot's direction-layer epilogue is still owed (kDirTmem)
-
-    for (long long slot = 0; slot < n_slots; ++slot) {
-      const long long pt_slot = tile_of(slot) * kTile + row;
-      float sig_part = 0.f;
-      // ---------------- trunk epilogues: D (TMEM) -> act -> A (TMEM)
-      const long long pt = pt_slot;
-      for (int l = 0; l < n_layers_epi; ++l) {
-        const float* bias = s.cst + CL.b[l];
-        const bool relu = true;
-#pragma unroll 1
-        for (int h = 0; h < 2; ++h) {
-          const bool tr = (p.debug & 8) && blockIdx.x == 0 && slot == 3 && tid == 0;
-          const int tb = 1024 + (l * 2 + h) * 8;
-          trace(tr, tb + 0);
-          mbar_wait(&s.d_full[h], (ph_d >> h) & 1); ph_d ^= 1u << h;
-          tc_fence_after();
-          trace(tr, tb + 1);
-          const int q = ch >> 1;                       // the 64-column quarter this thread's group belongs to
-          const int c0 = h * kNh + ch * 32;            // output columns == next layer's k
-          if (p.debug & 2) {
-            if (h == 0) { mbar_wait(&s.a_free, ph_free); ph_free ^= 1; }
-            tc_fence_before(); signal(&s.a_ready[h * 2 + q]); continue;
-          }
-          uint32_t v[32];
-          tmem_ld32(tbase + lane_base + kColD + c0, v);
-          tmem_wait_ld();
-          trace(tr, tb + 2);
-          // bias + activation + hi/lo split, in place: v[2j] = hi pair j, v[2j+1] = lo pair j
-          uint32_t mask_word = 0;        // kTrain == 2: [value > 0] of this thread's 32 columns, stored after the hand-off
-          auto finish_group = [&](auto relu_tag, auto sigma_tag) {
-            constexpr bool kRelu = decltype(relu_tag)::value, kSigma = decltype(sigma_tag)::value;
-            const float2* b2 = reinterpret_cast<const float2*>(bias + c0);
-            const float2* w2 = reinterpret_cast<const float2*>(s.cst + CL.sigma_w + c0);
-            const long long pt_block0 = pt - lane;      // first row of this warp's 32-row block
-            float* save_blk = kTrain == 1 ? p.save_h + ((size_t)l * p.n_points + pt_block0) * kWidth + c0 : nullptr;
-            float4 keep[4];
-            uint32_t h16[kTrain == 2 ? 16 : 1];      // this thread's 32 post-ReLU values as fp16 pairs
-            uint32_t mword = 0;                      // [value > 0] of the 32 columns (the fp32 test the reference's ReLU makes)
-#pragma unroll
-            for (int j = 0; j < 16; j += 2) {
-              float x[4];
-              if (kRelu && !kSigma && kTrain == 0) {
-                // nobody needs the fp32 post-activation value: ReLU and the fp16 range guard ride on the converts
-                // one 16-byte bias load and two packed fp32x2 adds (FADD2) per four columns
-                const float4 bb = *reinterpret_cast<const float4*>(b2 + j);
-                const float2 x01 = __fadd2_rn(make_float2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1])), make_float2(bb.x, bb.y));
-                const float2 x23 = __fadd2_rn(make_float2(__uint_as_float(v[2 * j + 2]), __uint_as_float(v[2 * j + 3])), make_float2(bb.z, bb.w));
-                split_pair_relu<kBf16, kSplit>(x01.x, x01.y, v[2 * j], v[2 * j + 1]);
-                split_pair_relu<kBf16, kSplit>(x23.x, x23.y, v[2 * j + 2], v[2 * j + 3]);
-                continue;
-              }
-              if (kTrain == 2 && !kSigma) {
-                // same sums, one 16-byte bias load and two packed adds per four columns (the training forward's epilogue is
-                // ~2.5x the inference one in instructions -- rn hi words, ReLU mask bits, activation stores -- and sets its pace)
-                const float4 bb = *reinterpret_cast<const float4*>(b2 + j);
-                const float2 x01 = __fadd2_rn(make_float2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1])), make_float2(bb.x, bb.y));
-                const float2 x23 = __fadd2_rn(make_float2(__uint_as_float(v[2 * j + 2]), __uint_as_float(v[2 * j + 3])), make_float2(bb.z, bb.w));
-                x[0] = x01.x; x[1] = x01.y; x[2] = x23.x; x[3] = x23.y;
-                if (kRelu) {
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) x[e] = fmaxf(x[e], 0.f);
-                }
-              } else {
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  const float2 bb = b2[j + e];
-                  x[2 * e] = __uint_as_float(v[2 * (j + e)]) + bb.x;
-                  x[2 * e + 1] = __uint_as_float(v[2 * (j + e) + 1]) + bb.y;
-                  if (kRelu) { x[2 * e] = fmaxf(x[2 * e], 0.f); x[2 * e + 1] = fmaxf(x[2 * e + 1], 0.f); }
-                  if (kSigma) {
-                    const float2 ww = w2[j + e];
-                    sig_part = fmaf(x[2 * e], ww.x, sig_part); sig_part = fmaf(x[2 * e + 1], ww.y, sig_part);
-                  }
-                }
-              }
-              if (kTrain == 1) {
-                keep[(j >> 1) & 3] = make_float4(x[0], x[1], x[2], x[3]);
-                if (((j >> 1) & 3) == 3) store_block16(keep, save_blk + (j >> 3) * 16, kWidth, pt_block0);
-              }
-              split_pair<kBf16, kSplit, kRelu>(x[0], x[1], v[2 * j], v[2 * j + 1]);
-              split_pair<kBf16, kSplit, kRelu>(x[2], x[3], v[2 * j + 2], v[2 * j + 3]);
-              if (kTrain == 2) {
-                // fp16 modes: the hi word of the split IS rn_fp16(value) (saturated); bf16 modes convert separately
-                h16[j] = kBf16 ? pack_half2_sat(x[0], x[1]) : v[2 * j];
-                h16[j + 1] = kBf16 ? pack_half2_sat(x[2], x[3]) : v[2 * j + 2];
-                // [x > 0] of the post-ReLU value (x >= +0; fmaxf(-0, +0) is +0): bits(x) + 0x7fffffff has its top bit set
-                // iff bits(x) != 0, and a funnel shift moves that bit in -- 2 instructions per column instead of 3 (compare,
-                // select, or).  Columns enter in ascending order, so the word is built bit-reversed (one BREV below).
-#pragma unroll
-                for (int e = 0; e < 4; ++e) mword = __funnelshift_l(__float_as_uint(x[e]) + 0x7fffffffu, mword, 1);
-              }
-            }
-            if (kTrain == 2) mword = __brev(mword);
-            if (kTrain == 2 && kBf16 && pt < p.ppad) {
-              const bool live = pt < p.n_points;
-              unsigned char* hb = p.a_h + (size_t)l * (size_t)p.ppad * (kWidth * 2);
-#pragma unroll
-              for (int c = 0; c < 4; ++c)
-                *reinterpret_cast<uint4*>(hb + a16_cell(pt, (c0 >> 3) + c, kWidth)) =
-                    live ? make_uint4(h16[4 * c], h16[4 * c + 1], h16[4 * c + 2], h16[4 * c + 3]) : make_uint4(0u, 0u, 0u, 0u);
-            }
-            mask_word = mword;
-          };
-          if (l == 7) finish_group(std::true_type{}, std::true_type{});
-          else finish_group(std::true_type{}, std::false_type{});
-          // half a's results go to A[k 0..127], which this layer's (b,k0) MMAs still read: the math above
-          // overlaps both b phases, the stores wait until those MMAs have retired (a_free); half b's
-          // target A[k 128..255] is idle
-          if (h == 0) { mbar_wait(&s.a_free, ph_free); ph_free ^= 1; tc_fence_after(); }
-          {
-            uint32_t phi[16], plo[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) { phi[j] = v[2 * j]; plo[j] = v[2 * j + 1]; }
-            tmem_st16(tbase + lane_base + kColAhi + (c0 >> 1), phi);
-            if (kSplit) tmem_st16(tbase + lane_base + kColAlo + (c0 >> 1), plo);
-            tmem_wait_st();
-            tc_fence_before();
-            signal(&s.a_ready[h * 2 + q]);
-            trace(tr, tb + 3 + q);
-            if (kTrain == 2 && pt < p.ppad) {
-              // what the backward reads -- off the layer-to-layer critical path, after the hand-off.  fp16 modes: the saved
-              // activation IS the hi word just stored to TMEM (rn_fp16 of the saturated value); bf16 modes stored theirs above
-              const bool live = pt < p.n_points;
-              if (!kBf16) {
-                unsigned char* hb = p.a_h + (size_t)l * (size_t)p.ppad * (kWidth * 2);
-#pragma unroll
-                for (int c = 0; c < 4; ++c)
-                  *reinterpret_cast<uint4*>(hb + a16_cell(pt, (c0 >> 3) + c, kWidth)) =
-                      live ? make_uint4(phi[4 * c], phi[4 * c + 1], phi[4 * c + 2], phi[4 * c + 3]) : make_uint4(0u, 0u, 0u, 0u);
-              }
-              p.a_mask[a16_mask_index(l, c0 >> 5, pt, p.ppad)] = live ? mask_word : 0u;
-            }
-          }
-        }
-        // ---- background work in the idle window before this layer's next accumulator half is ready
-        if (kDirTmem && pending && l < kDirPieces) {
-          // the previous tile's direction-layer epilogue, one piece per layer; sigp[0] still holds that tile's sigma
-          // (rewritten at l == 7 of this slot)
-          const bool trp = (p.debug & 8) && blockIdx.x == 0 && slot == 4 && tid == 0;
-          const long long dpt = tile_of(slot - 1) * kTile + row;
-          if (l == 0) trace(trp, 1024 + 18 * 8 + 5);
-          dir_piece(l, dpt, nullptr);
-          if (l == kDirPieces - 1) {
-            trace(trp, 1024 + 18 * 8 + 3);
-            dir_finish(dpt);
-            pending = false;
-            trace(trp, 1024 + 18 * 8 + 4);
-          }
-        }
-        if (l == 7) {
-          // sigma head (nerf.py:136): combine the two column halves of each row
-          s.sigp[ch][row] = sig_part;
-          epi_bar_sync();
-          if (ch == 0) {
-            const float sg = ((s.sigp[0][row] + s.sigp[1][row]) + (s.sigp[2][row] + s.sigp[3][row])) + s.cst[CL.sigma_b];
-            s.sigp[0][row] = sg;         // keep for the final float4
-            if (p.sigma_only && pt < p.n_points) p.out[pt] = sg;
-          }
-          epi_bar_sync();
-        }
-      }
-      if (p.sigma_only) continue;
-
-      // ---------------- direction layer: accumulator full -> (drain) -> epilogue now or in the next slot
-      {
-        const bool tr = (p.debug & 8) && blockIdx.x == 0 && slot == 3 && tid == 0;
-        const int tb = 1024 + 18 * 8;
-        trace(tr, tb + 0);
-        if (kDirTmem) { mbar_wait(&s.d_full_dir, (uint32_t)slot & 1); }
-        else { mbar_wait(&s.d_full[0], ph_d & 1); ph_d ^= 1u; }
-        tc_fence_after();
-        trace(tr, tb + 1);
-        if (kDirTmem) {
-          pending = true;            // the accumulator is columns [384,512): nothing to drain
-        } else {
-          uint32_t v[32];
-          tmem_ld32(tbase + lane_base + kColD + cdir0, v);
-          tmem_wait_ld();
-          tc_fence_before();
-          signal(&s.d_drained);      // D[0,128) is in registers: the next slot's layer 1 may overwrite it
-          trace(tr, tb + 2);
-          dir_piece(0, pt_slot, v);
-          trace(tr, tb + 3);
-          dir_finish(pt_slot);
-          trace(tr, tb + 4);
-        }
-        if (kDirTmem) trace(tr, tb + 2);
-      }
-    }
-    if (kDirTmem && pending) {     // the last slot's direction-layer epilogue
-      const long long dpt = tile_of(n_slots - 1) * kTile + row;
-#pragma unroll 1
-      for (int pc = 0; pc < kDirPieces; ++pc) dir_piece(pc, dpt, nullptr);
-      dir_finish(dpt);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (kCg == 2) cluster_sync_all();   // neither CTA leaves (or frees TMEM) while its peer may still touch it
-  if (warp == kMmaWarp) { if (kCg == 2) tmem_dealloc_pair(tbase); else tmem_dealloc<512>(tbase); }
 }
 
 // ------------------------------------------------------------------ host
-template <bool kBf16, bool kSplit, bool kEmbedded, int kCg, int kTrain = 0>
+template <bool kBf16, bool kSplit, bool kEmbedded, int kTrain = 0>
 static int launch_tc(const TcParams& p, cudaStream_t st) {
   static SmemOptIn optin;
   const long long ntiles = (p.n_points + kTile - 1) / kTile;
   if (ntiles == 0) return SNB_OK;       // an empty pass is a no-op: no CUDA call at all
-  const size_t smem = sizeof(TcSmem<kSplit, kCg, kTrain>) + 1024;
-  auto kern = field_tc_kernel<kBf16, kSplit, kEmbedded, kCg, kTrain>;
+  const size_t smem = sizeof(TcSmem<kSplit>) + 1024;
+  auto kern = field_tc_kernel<kBf16, kSplit, kEmbedded, kTrain>;
   if (int rc = ensure_smem(kern, optin, (int)smem, "field_tc")) return rc;
-  const int sms = sm_count();
-  long long groups = (ntiles + kCg - 1) / kCg;
-  if (groups > sms / kCg) groups = sms / kCg;
-  static const int debug = getenv("SNB_TC_DEBUG") ? atoi(getenv("SNB_TC_DEBUG")) : 0;
-  TcParams pd = p;
-  pd.debug = debug;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(groups * kCg));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kCg;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, pd);
-  if (e != cudaSuccess) return fail(SNB_ERR_CUDA, "field_tc_kernel launch: %s", cudaGetErrorString(e));
+  long long ctas = sm_count();
+  if (ctas > ntiles) ctas = ntiles;
+  kern<<<(unsigned)ctas, kThreads, smem, st>>>(p);
   return check_launch("field_tc_kernel");
-}
-
-template <bool kBf16, bool kSplit, bool kEmbedded>
-static int launch_tc_cg(const TcParams& p, cudaStream_t st) {
-  return launch_tc<kBf16, kSplit, kEmbedded, 2>(p, st);
 }
 
 template <bool kEmbedded>
 static int dispatch_tc(int precision, const TcParams& p, cudaStream_t st) {
   switch (precision) {
-    case SNB_PREC_F16X3: return launch_tc_cg<false, true, kEmbedded>(p, st);
-    case SNB_PREC_BF16X3: return launch_tc_cg<true, true, kEmbedded>(p, st);
-    case SNB_PREC_BF16: return launch_tc_cg<true, false, kEmbedded>(p, st);
+    case SNB_PREC_F16X3: return launch_tc<false, true, kEmbedded>(p, st);
+    case SNB_PREC_BF16X3: return launch_tc<true, true, kEmbedded>(p, st);
+    case SNB_PREC_BF16: return launch_tc<true, false, kEmbedded>(p, st);
   }
   return fail(SNB_ERR_INVALID, "precision %d is not a tensor-core mode", precision);
 }
@@ -1248,9 +756,9 @@ int field_forward_train_tc(const void* packed, int precision, const float* rays,
   p.out = raw;
   p.save_enc = save_enc; p.save_dir = save_dir; p.save_h = save_h; p.save_g = save_g;
   switch (precision) {
-    case SNB_PREC_F16X3: return launch_tc<false, true, false, 2, 1>(p, st);
-    case SNB_PREC_BF16X3: return launch_tc<true, true, false, 2, 1>(p, st);
-    case SNB_PREC_BF16: return launch_tc<true, false, false, 2, 1>(p, st);
+    case SNB_PREC_F16X3: return launch_tc<false, true, false, 1>(p, st);
+    case SNB_PREC_BF16X3: return launch_tc<true, true, false, 1>(p, st);
+    case SNB_PREC_BF16: return launch_tc<true, false, false, 1>(p, st);
   }
   return fail(SNB_ERR_INVALID, "precision %d is not a tensor-core mode", precision);
 }
@@ -1269,9 +777,9 @@ int field_forward_train16_tc(const void* packed, int precision, const float* ray
   p.a_mask = reinterpret_cast<uint32_t*>(b + L.mask);
   p.ppad = a16_pad(p.n_points);
   switch (precision) {
-    case SNB_PREC_F16X3: return launch_tc<false, true, false, 2, 2>(p, st);
-    case SNB_PREC_BF16X3: return launch_tc<true, true, false, 2, 2>(p, st);
-    case SNB_PREC_BF16: return launch_tc<true, false, false, 2, 2>(p, st);
+    case SNB_PREC_F16X3: return launch_tc<false, true, false, 2>(p, st);
+    case SNB_PREC_BF16X3: return launch_tc<true, true, false, 2>(p, st);
+    case SNB_PREC_BF16: return launch_tc<true, false, false, 2>(p, st);
   }
   return fail(SNB_ERR_INVALID, "precision %d is not a tensor-core mode", precision);
 }
@@ -1288,9 +796,3 @@ int mlp_forward_tc(const void* packed, int precision, const float* x, int64_t x_
 }
 
 }  // namespace snb
-
-// debug-only export (not part of the public header): copy the device trace buffer to the host
-extern "C" int snb_debug_trace(long long* host_out, int n) {
-  if (n > snb::kTraceLen) n = snb::kTraceLen;
-  return cudaMemcpyFromSymbol(host_out, snb::g_trace, sizeof(long long) * n) == cudaSuccess ? 0 : -2;
-}

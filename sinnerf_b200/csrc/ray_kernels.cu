@@ -840,10 +840,13 @@ __global__ void __launch_bounds__(128) importance_merge_kernel(
 // image header (snb_refresh_weights).  2.4 MB of L2/HBM reads, one launch; the last block to finish
 // compares, sets header.dirty and resets the scratch fields.
 // ---------------------------------------------------------------------------------------
-// Grid: 148 blocks x 1024 threads, four words per thread.  (Round 2 launched 64 x 256 -- 36 words per thread, 29 us
-// per model, i.e. 58 us of the 900 us configs[2] patch render, profiles/r02b_timeline_patch_bf16_before.txt; 582 x 256
-// blocks took 16 us: two same-address atomics per block serialise at ~13 ns each.)
-constexpr int kCheckBlocks = 148, kCheckThreads = 1024;
+// Grid: 146 blocks x 1024 threads, four words per thread: the smallest grid of 1024-thread blocks that covers the
+// 595 844 parameter words in one pass (146 x 4096 = 598 016; static_assert below).  (Fewer threads with more words each serialise load latencies; more, smaller
+// blocks add same-address atomics, two per block.)
+constexpr int kCheckBlocks = 146, kCheckThreads = 1024;
+static_assert(kCheckBlocks * kCheckThreads * 4 >= SNB_PARAM_FLOATS &&
+                  (kCheckBlocks - 1) * kCheckThreads * 4 < SNB_PARAM_FLOATS,
+              "params_check_kernel: smallest one-pass grid");
 __device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
   x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
   x ^= x >> 27; x *= 0x94d049bb133111ebull;

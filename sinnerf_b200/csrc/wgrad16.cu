@@ -6,49 +6,39 @@
 //
 // (reference: autograd of `nn.Linear` inside models/nerf.py:105-148.)  dY, X and hg are fp16 tensors in
 // the T32 layout: a 32-point tile copied verbatim into shared memory IS the MN-major SWIZZLE_NONE canonical
-// operand of tcgen05.mma (probes/umma_mn_probe.cu), so the whole kernel is
-//   producer (1 elected thread)   cp.async.bulk of the tile's dY block (FA x 64 B) and X block (FB x 64 B)
+// wgmma operand, so the whole kernel is
+//   producer (thread 0)           cp.async.bulk of the tile's dY block (128 features x 64 B) and X block (FB x 64 B)
 //                                 into a kStages-deep ring (mbarrier complete_tx);
-//   issuer   (1 elected thread)   per tile 2 K-steps (K = 16 points) x NM out-feature blocks of
-//                                 tcgen05.mma SS  M = 128, N = FB  into TMEM accumulators that live for the
-//                                 CTA's whole slice of points; one product (fp16 x fp16, fp32 accumulate);
-//   bias / epilogue (4 warps)     column sums of the dY tile straight from shared memory (lane = point,
-//                                 8 features per 16-byte cell) while the MMAs run; at the end TMEM ->
-//                                 smem -> scaled, coalesced fp32 vector atomics (split-P reduction).
+//   two warpgroups                per tile 2 K-steps (K = 16 points) of wgmma SS, M = 64 out features each,
+//                                 N = FB, into register accumulators that live for the CTA's whole slice of
+//                                 points; one product (fp16 x fp16, fp32 accumulate); column sums of the dY tile
+//                                 (the bias gradient) from shared memory while the MMAs run; at the end scaled
+//                                 fp32 reductions from the fragments (split-P reduction; column pairs as red.v2).
 // No converter warps, no transposition, every HBM byte read once: 2 (FA + FB) bytes per point
 // (1 KB for a 256 x 256 layer; the fp32 version moved 2 KB and converted all of it in registers).
-// Roofline: HBM.  Shared-memory traffic per tile (TMA write + 2 NM operand reads + bias read) is the second
-// limit, the tensor pipe (2 NM MMAs of ~160 cycles per 32 points) the third.
+// Roofline: HBM (the fp32 reductions of the epilogue are per CTA, independent of the number of points).
 #include "act16.cuh"
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace snb {
-using namespace umma;
+using namespace wg;
 
 namespace {
 
-constexpr int kW16EpiWarps = 4;
-constexpr int kW16LoadWarp = kW16EpiWarps, kW16MmaWarp = kW16EpiWarps + 1;
-constexpr int kW16Threads = (kW16EpiWarps + 2) * 32;
+constexpr int kW16Threads = 256;   // two warpgroups: out-feature rows [64 w, +64) of the CTA's 128-row block
 
 // NM: 128-row out-feature blocks of dY (FA = 128 NM; 0 = head rows only); FB: X features (MMA N); kHead: hg operand
 template <int NM, int FB, bool kHead>
 struct W16Geo {
   static constexpr int kFA = 128 * NM;
-  static constexpr int kDyBytes = kFA * 64, kXBytes = FB * 64, kHgBytes = kHead ? 512 : 0;
+  static constexpr int kDyBytes = 128 * 64, kXBytes = FB * 64, kHgBytes = kHead ? 512 : 0;   // per 32-point tile
   static constexpr int kStageBytes = kDyBytes + kXBytes + kHgBytes;
   static constexpr int kStagesRaw = (160 * 1024) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kOutLd = FB + 4;
-  static constexpr int kOutBytes = 128 * kOutLd * 4;                   // epilogue staging, aliases the ring
-  static constexpr int kRingBytes = kStages * kStageBytes;
-  static constexpr int kSmemBytes = (kRingBytes > kOutBytes ? kRingBytes : kOutBytes) + 1024;
-  static constexpr int kAccCols = (NM + (kHead ? 1 : 0)) * FB;
-  static constexpr int kTmemCols = kAccCols <= 32 ? 32 : (kAccCols <= 64 ? 64 : (kAccCols <= 128 ? 128 : (kAccCols <= 256 ? 256 : 512)));
-  static_assert(kAccCols <= 512, "TMEM columns");
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024;
   static_assert(kStages >= 2 && kSmemBytes <= 227 * 1024, "shared memory");
-  static_assert(FB % 16 == 0 && FB >= 16 && FB <= 256, "MMA N");
+  static_assert(FB == 32 || FB == 64 || FB == 128 || FB == 256, "MMA N");
 };
 
 struct W16Args {
@@ -59,191 +49,144 @@ struct W16Args {
   float* dW; int ldw; int col_off;
   float* db;                   // nullable
   const float* scale;          // device: dY is stored as true * (*scale)
-  float* dH[8]; int ldh;       // kHead: destination row pointers (nullable per row), row stride unused (rows are separate tensors)
+  float* dH[8];                // kHead: destination row pointers (nullable per row)
   const float* scale2;         // device: scale of hg
   long long n_tiles;           // 32-point tiles (Ppad / 32)
   long long tiles_per_cta;
 };
 
-__host__ __device__ constexpr uint32_t idesc_mn_f16(uint32_t M, uint32_t N) {
-  // kind::f16, fp16 x fp16 -> fp32, A and B MN-major
-  return (1u << 4) | (0u << 7) | (0u << 10) | (1u << 15) | (1u << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
+template <int FB>
+__device__ __forceinline__ void wgmma_mn(float (&d)[FB / 2], uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (FB == 256) wgmma_m64n256_f16_mn(d, a, b, acc);
+  else if constexpr (FB == 128) wgmma_m64n128_f16_mn(d, a, b, acc);
+  else if constexpr (FB == 64) wgmma_m64n64_f16_mn(d, a, b, acc);
+  else wgmma_m64n32_f16_mn(d, a, b, acc);
 }
 
+// CTA (x, y): out-feature block y (y == NM: the head rows) over the 32-point tiles of slice x.  Thread 0 bulk-copies
+// each tile's dY block (128 features x 32 points = 8 KB, contiguous in T32) and X (FB x 64 B) into a ring; a tile
+// copied verbatim IS the MN-major SWIZZLE_NONE canonical operand (LBO = 128 B: next 8 points, SBO = 512 B: next 8
+// features).  wgmma M = 64 out features per warpgroup, N = FB in features, K = 16 points; the accumulators live in
+// registers for the CTA's whole slice; epilogue: scaled fp32 reductions straight from the fragments (column pairs
+// as one red.v2 where the address is 8-byte aligned).
 template <int NM, int FB, bool kHead>
 __global__ void __launch_bounds__(kW16Threads, 1) wgrad16_kernel(W16Args a) {
   using G = W16Geo<NM, FB, kHead>;
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  extern __shared__ unsigned char smem_raw[];
   unsigned char* ring = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ uint64_t full[G::kStages], empty[G::kStages], d_full;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t full[G::kStages], empty[G::kStages];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int mb = blockIdx.y;
+  const bool head = kHead && mb == NM;
   const long long t_begin = (long long)blockIdx.x * a.tiles_per_cta;
   const long long t_end = t_begin + a.tiles_per_cta < a.n_tiles ? t_begin + a.tiles_per_cta : a.n_tiles;
   const int n_my = t_end > t_begin ? (int)(t_end - t_begin) : 0;
+  if (n_my == 0) return;
 
   if (tid == 0) {
-    for (int i = 0; i < G::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1 + (NM > 0 ? kW16EpiWarps * 32 : 0)); }
-    mbar_init(&d_full, 1);
+    for (int i = 0; i < G::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kW16Threads / 32); }
     fence_mbar_init();
   }
-  if (warp == kW16MmaWarp) tmem_alloc<G::kTmemCols>(&tmem_base_s);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tbase = tmem_base_s;
+  int next_load = 0;
+  auto produce = [&](int upto) {
+    for (; next_load < n_my && next_load < upto; ++next_load) {
+      const int st = next_load % G::kStages;
+      mbar_wait(&empty[st], ((next_load / G::kStages) & 1) ^ 1);
+      unsigned char* dst = ring + (size_t)st * G::kStageBytes;
+      const long long t = t_begin + next_load;
+      const uint32_t bytes = (head ? 512 : G::kDyBytes) + G::kXBytes;
+      mbar_arrive_expect_tx(&full[st], bytes);
+      if (head) bulk_g2s(dst, a.hg + (size_t)t * 512, 512, &full[st]);
+      else bulk_g2s(dst, a.dY + ((size_t)t * (G::kFA / 8) + mb * 16) * 512, G::kDyBytes, &full[st]);
+      for (int o = 0; o < G::kXBytes; o += 16384)
+        bulk_g2s(dst + G::kDyBytes + o, a.X + (size_t)t * G::kXBytes + o, G::kXBytes - o < 16384 ? G::kXBytes - o : 16384, &full[st]);
+    }
+  };
+  if (tid == 0) produce(G::kStages);
+  __syncwarp();
 
-  if (warp == kW16LoadWarp) {
-    // ======================= producer: one tile = two (three) contiguous runs in HBM =======================
-    if (elect_one()) {
-      for (int i = 0; i < n_my; ++i) {
-        const int st = i % G::kStages;
-        mbar_wait(&empty[st], ((i / G::kStages) & 1) ^ 1);
-        unsigned char* dst = ring + (size_t)st * G::kStageBytes;
-        const long long t = t_begin + i;
-        mbar_arrive_expect_tx(&full[st], (uint32_t)G::kStageBytes);
-        if (NM > 0) {
-          const unsigned char* src = a.dY + (size_t)t * G::kDyBytes;
-          for (int o = 0; o < G::kDyBytes; o += 16384) bulk_g2s(dst + o, src + o, G::kDyBytes - o < 16384 ? G::kDyBytes - o : 16384, &full[st]);
+  const int wgi = warp >> 2, wq = warp & 3, g = lane >> 2, tq = lane & 3;
+  // bias: thread = (feature group tid / 16 of this block, points 2 (tid % 16) + {0, 1} of every tile)
+  float bs[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) bs[j] = 0.f;
+  const bool do_bias = !head && a.db != nullptr;
+  float acc[FB / 2];
+#pragma unroll
+  for (int i = 0; i < FB / 2; ++i) acc[i] = 0.f;
+  int pend = -1;
+  for (int i = 0; i < n_my; ++i) {
+    const int st = i % G::kStages;
+    mbar_wait(&full[st], (i / G::kStages) & 1);
+    const unsigned char* tile = ring + (size_t)st * G::kStageBytes;
+    const uint32_t base = smem_u32(tile);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+      // head rows: the 8 head-gradient features as all 8 row groups of A (SBO = 0): rows 8..63 repeat rows 0..7
+      const uint64_t ad = head ? make_smem_desc(base + ks * 256, 128, 0)
+                               : make_smem_desc(base + wgi * (8 * 512) + ks * 256, 128, 512);
+      const uint64_t bd = make_smem_desc(base + G::kDyBytes + ks * 256, 128, 512);
+      wgmma_mn<FB>(acc, ad, bd, (i > 0 || ks > 0) ? 1u : 0u);
+    }
+    wgmma_commit();
+    if (do_bias) {
+      const int grp = tid >> 4, p2 = (tid & 15) * 2;
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const uint4 c = *reinterpret_cast<const uint4*>(tile + grp * 512 + (p2 + q) * 16);
+        const uint32_t w[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[j]));
+          bs[2 * j] += f.x; bs[2 * j + 1] += f.y;
         }
-        {
-          const unsigned char* src = a.X + (size_t)t * G::kXBytes;
-          for (int o = 0; o < G::kXBytes; o += 16384)
-            bulk_g2s(dst + G::kDyBytes + o, src + o, G::kXBytes - o < 16384 ? G::kXBytes - o : 16384, &full[st]);
-        }
-        if (kHead) bulk_g2s(dst + G::kDyBytes + G::kXBytes, a.hg + (size_t)t * 512, 512, &full[st]);
       }
     }
+    wgmma_wait<1>();
+    if (pend >= 0 && lane == 0) mbar_arrive(&empty[pend]);
+    pend = st;
+    if (tid == 0) produce(i + G::kStages);
     __syncwarp();
-  } else if (warp == kW16MmaWarp) {
-    // ======================= MMA issuer =======================
-    if (elect_one()) {
-      constexpr uint32_t idesc = idesc_mn_f16(128, FB);
-      for (int i = 0; i < n_my; ++i) {
-        const int st = i % G::kStages;
-        mbar_wait(&full[st], (i / G::kStages) & 1);
-        tc_fence_after();
-        const uint32_t base = smem_u32(ring + (size_t)st * G::kStageBytes);
+  }
+  wgmma_wait<0>();
+
+  const float inv = head ? 1.0f / __ldg(a.scale2) : 1.0f / __ldg(a.scale);
+  if (do_bias) {
 #pragma unroll
-        for (int ks = 0; ks < 2; ++ks) {
-          // K step = 16 points = 256 B along the point axis; LBO (next 8 points) 128 B, SBO (next 8 features) 512 B
-          const uint64_t bd = make_smem_desc(base + G::kDyBytes + ks * 256, 128, 512);
-          const uint32_t acc = (i > 0 || ks > 0) ? 1u : 0u;
+    for (int j = 0; j < 8; ++j) {
+      float v = bs[j];
 #pragma unroll
-          for (int mb = 0; mb < NM; ++mb) {
-            const uint64_t ad = make_smem_desc(base + mb * (128 * 64) + ks * 256, 128, 512);
-            mma_ss(tbase + mb * FB, ad, bd, idesc, acc);
-          }
-          if (kHead) {
-            // the 8 head-gradient features as all 16 row groups of A (SBO = 0): rows 8..127 of the result repeat rows 0..7
-            const uint64_t ad = make_smem_desc(base + G::kDyBytes + G::kXBytes + ks * 256, 128, 0);
-            mma_ss(tbase + NM * FB, ad, bd, idesc, acc);
-          }
-        }
-        mma_commit(&empty[st]);
-      }
-      mma_commit(&d_full);
-    }
-    __syncwarp();
-  } else {
-    // ======================= bias: column sums of dY from the staged tiles =======================
-    // warp w owns feature groups [w * kGw, +kGw); lane = point.  acc[g][j] = partial sum over this lane's points.
-    constexpr int kGw = NM > 0 ? (G::kFA / 8) / kW16EpiWarps : 1;
-    float acc[kGw][8];
-#pragma unroll
-    for (int g = 0; g < kGw; ++g)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[g][j] = 0.f;
-    if (NM > 0) {
-      for (int i = 0; i < n_my; ++i) {
-        const int st = i % G::kStages;
-        mbar_wait(&full[st], (i / G::kStages) & 1);
-        if (a.db != nullptr) {
-          const unsigned char* tile = ring + (size_t)st * G::kStageBytes;
-#pragma unroll
-          for (int g = 0; g < kGw; ++g) {
-            const uint4 c = *reinterpret_cast<const uint4*>(tile + (warp * kGw + g) * 512 + lane * 16);
-            const uint32_t w[4] = {c.x, c.y, c.z, c.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[j]));
-              acc[g][2 * j] += f.x; acc[g][2 * j + 1] += f.y;
-            }
-          }
-        }
-        mbar_arrive(&empty[st]);
-      }
-    }
-    const float inv = (NM > 0 || !kHead) ? 1.0f / __ldg(a.scale) : 1.0f;
-    if (NM > 0 && a.db != nullptr && n_my > 0) {
-#pragma unroll
-      for (int g = 0; g < kGw; ++g)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float v = acc[g][j];
-#pragma unroll
-          for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-          if (lane == ((g * 8 + j) & 31)) atomicAdd(a.db + (warp * kGw + g) * 8 + j, v * inv);
-        }
-    }
-    // ======================= epilogue: TMEM -> smem -> scaled atomics =======================
-    // (the staging buffer aliases the ring: every warp must be done reading tiles before anyone writes it)
-    asm volatile("bar.sync 1, %0;" ::"n"(kW16EpiWarps * 32) : "memory");
-    if (n_my > 0) {
-      mbar_wait(&d_full, 0);
-      tc_fence_after();
-      float* out = reinterpret_cast<float*>(ring);        // [128][FB + 4]; every copy and MMA has retired
-      constexpr int kLd = G::kOutLd;
-      constexpr int kBlocks = NM + (kHead ? 1 : 0);
-#pragma unroll 1
-      for (int mb = 0; mb < kBlocks; ++mb) {
-        const bool head = kHead && mb == NM;
-        const float sc = head ? 1.0f / __ldg(a.scale2) : inv;
-        const int rows = head ? 8 : 128;                  // head block: only its first 8 rows are distinct
-        if (warp * 32 < rows) {
-          const int row = warp * 32 + lane;
-#pragma unroll 1
-          for (int c0 = 0; c0 < FB; c0 += 32) {
-            uint32_t v[32];
-            tmem_ld32(tbase + ((uint32_t)(warp * 32) << 16) + mb * FB + c0, v);
-            tmem_wait_ld();
-            if (row < rows) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                *reinterpret_cast<float4*>(out + row * kLd + c0 + j) =
-                    make_float4(__uint_as_float(v[j]) * sc, __uint_as_float(v[j + 1]) * sc, __uint_as_float(v[j + 2]) * sc,
-                                __uint_as_float(v[j + 3]) * sc);
-            }
-          }
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kW16EpiWarps * 32) : "memory");
-        if (head) {
-          // features 4..7 of the hg cell are the fp16 residuals of features 0..3: row r + row r + 4
-          for (int e = tid; e < 4 * FB; e += kW16EpiWarps * 32) {
-            const int r = e / FB, k = e - r * FB;
-            if (a.dH[r] != nullptr && k < a.K) atomicAdd(a.dH[r] + k, out[r * kLd + k] + out[(r + 4) * kLd + k]);
-          }
-        } else if (a.K == FB && ((a.ldw | a.col_off) & 3) == 0 && (reinterpret_cast<uintptr_t>(a.dW) & 15) == 0) {
-          for (int e = tid; e < 128 * (FB / 4); e += kW16EpiWarps * 32) {
-            const int m = e / (FB / 4), k = (e - m * (FB / 4)) * 4;
-            const float4 v = *reinterpret_cast<const float4*>(out + m * kLd + k);
-            float* dst = a.dW + (size_t)(mb * 128 + m) * a.ldw + a.col_off + k;
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-                         : "memory");
-          }
-        } else {
-          for (int e = tid; e < 128 * FB; e += kW16EpiWarps * 32) {
-            const int m = e / FB, k = e - m * FB;
-            if (k < a.K) atomicAdd(a.dW + (size_t)(mb * 128 + m) * a.ldw + a.col_off + k, out[m * kLd + k]);
-          }
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kW16EpiWarps * 32) : "memory");
-      }
+      for (int off = 8; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+      if ((tid & 15) == 0) atomicAdd(a.db + mb * 128 + (tid >> 4) * 8 + j, v * inv);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kW16MmaWarp) tmem_dealloc<G::kTmemCols>(tbase);
+  // ---- epilogue: fragments -> scaled fp32 atomics
+  if (head) {
+    // features 4..7 of the hg cell are the fp16 residuals of features 0..3: row r + row r + 4 (lane + 16)
+    if (wgi == 0 && wq == 0) {
+#pragma unroll
+      for (int j = 0; j < FB / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float v = acc[4 * j + e] + __shfl_down_sync(0xffffffffu, acc[4 * j + e], 16);
+          const int k = 8 * j + 2 * tq + e;
+          if (g < 4 && a.dH[g] != nullptr && k < a.K) atomicAdd(a.dH[g] + k, v * inv);
+        }
+    }
+    return;
+  }
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int m = mb * 128 + wgi * 64 + wq * 16 + g + 8 * rr;
+    float* dst = a.dW + (size_t)m * a.ldw + a.col_off;
+#pragma unroll
+    for (int j = 0; j < FB / 8; ++j) {
+      const int k = 8 * j + 2 * tq;
+      if (k < a.K) red_add_pair(dst + k, acc[4 * j + 2 * rr] * inv, acc[4 * j + 2 * rr + 1] * inv, k + 1 < a.K);
+    }
+  }
 }
 
 template <int NM, int FB, bool kHead>
@@ -251,11 +194,12 @@ int launch_wgrad16(W16Args a, cudaStream_t st) {
   using G = W16Geo<NM, FB, kHead>;
   static SmemOptIn optin;
   if (int rc = ensure_smem(wgrad16_kernel<NM, FB, kHead>, optin, G::kSmemBytes, "wgrad16")) return rc;
-  long long ctas = sm_count();
+  const int blocks = NM + (kHead ? 1 : 0);
+  long long ctas = (sm_count() + blocks - 1) / blocks;
   if (ctas > a.n_tiles) ctas = a.n_tiles;
   a.tiles_per_cta = (a.n_tiles + ctas - 1) / ctas;
   ctas = (a.n_tiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
-  wgrad16_kernel<NM, FB, kHead><<<(unsigned)ctas, kW16Threads, G::kSmemBytes, st>>>(a);
+  wgrad16_kernel<NM, FB, kHead><<<dim3((unsigned)ctas, blocks), kW16Threads, G::kSmemBytes, st>>>(a);
   return check_launch("wgrad16_kernel");
 }
 

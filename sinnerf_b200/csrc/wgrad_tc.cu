@@ -1,305 +1,230 @@
-// wgrad_tc.cu -- weight gradients of one nn.Linear on 5th-gen tensor cores.
+// wgrad_tc.cu -- weight gradients of one nn.Linear from fp32 row-major operands, on Hopper tensor cores.
 //
 //   dW[n][col_off + k] += sum_p dY[p][n] * X[p][k]      db[n] += sum_p dY[p][n]
 //
 // (reference: autograd of `nn.Linear` inside models/nerf.py:105-148; the SIMT version of the same
 // contraction is wgrad_kernel in field_bwd.cu.)  dY (P, N) and X (P, ldx) are the plain row-major
-// fp32 tensors the training forward / the dgrad chain leave in HBM.
+// fp32 tensors the fp32-storage training forward / dgrad chain leave in HBM.
 //
 // As an MMA the reduction runs over POINTS:  D[m = out feature][n' = in feature] += A[m][p] B[n'][p],
-// so both operands are needed "points-major" -- the transpose of how they sit in HBM -- and as bf16
-// hi + lo planes (gradients span fp32's exponent range; the 3-product split  x*w ~ xh*wh + xl*wh +
-// xh*wl  keeps ~16 mantissa bits per operand, the gradient parity bar is 1e-3 per tensor).
+// and both operands enter as bf16 hi + lo planes (gradients span fp32's exponent range; the 3-product
+// split  x*w ~ xh*wh + xl*wh + xh*wl  keeps ~16 significand bits per operand, the gradient parity bar is
+// 1e-3 per tensor).
 //
-// A CTA owns a slice of points and ALL out features, so every byte of dY and X is read from HBM
-// exactly once (2 KB per point for a 256x256 layer):
-//   producer  (1 elected thread)  16 points of dY and of X are two contiguous runs in HBM: two
-//             cp.async.bulk copies per batch into a 4-deep raw fp32 ring (mbarrier complete_tx);
-//   converters (8 warps)          a thread owns one feature and 8 consecutive points: 8 conflict-free
-//             LDS from the raw tile, split, one 16-byte row of the K-major (SWIZZLE_NONE) core-matrix
-//             layout for the hi plane and one for the lo plane -- the transpose costs nothing extra;
-//             also the bias gradient (column sums) and, for the dgrad that follows, [X > 0] as one
-//             32-bit word per point and 32 features (a warp ballot);
-//   issuer    (1 elected thread)  tcgen05.mma SS, M = 128 per out-feature block, N = Kpad, K = 16
-//             points, 3 products, into TMEM accumulators that live for the whole slice (up to
-//             2 x 256 = all 512 columns);
-//   epilogue  TMEM -> smem -> coalesced fp32 atomics (split-P reduction across CTAs).
-// Roofline: HBM, 4 (N + K) bytes per point; shared-memory traffic (TMA in, LDS, STS, MMA operand
-// reads: ~10.5 KB per point) is the second limit, the tensor pipe (3 x 160 cycles per 16 points and
-// out-feature block) the third; see DESIGN.md.
+// CTA (x, y): the 32-point tiles of slice x, out-feature block y (128 rows).  Per tile, all 256 threads
+// load the fp32 rows (16-byte loads), split them and store 16-byte cells of the T32 layout (act16.cuh) --
+// a cell is 8 features of one point, so a tile in shared memory IS the MN-major SWIZZLE_NONE canonical
+// wgmma operand (LBO 128 B: next 8 points, SBO 512 B: next 8 features).  Two tile buffers: the conversion
+// of tile i overlaps the wgmmas of tile i - 1.  Two warpgroups (M = 64 out features each, N = in features,
+// K = 16 points) accumulate in registers for the whole slice; the same pass sums the bias gradient in fp32
+// and, for the dgrad that follows, emits [X > 0] as (P, 8) words.  Epilogue: fp32 reductions from the
+// fragments (split-P reduction), pairs of columns as one red.v2 where aligned.
+// Roofline: HBM, 4 (N + K) bytes per point (X is read once per out-feature block).
 #include <cuda_bf16.h>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace snb {
-using namespace umma;
+using namespace wg;
 
 namespace {
 
-constexpr int kWgBatch = 16;             // points per batch = one MMA K step
-constexpr int kWgConvWarps = 8;
-constexpr int kWgMmaWarp = kWgConvWarps, kWgLoadWarp = kWgConvWarps + 1;
-constexpr int kWgThreads = (kWgConvWarps + 2) * 32;
-constexpr int kWgRawStages = 4, kWgPlaneBufs = 2;
+constexpr int kWtThreads = 256;
 
-// KP: in features padded to an MMA N (256 / 64 / 32); NM: 128-row out-feature blocks (N = 128 NM); LDX: X row length
-template <int KP, int NM, int LDX>
-struct WgGeo {
-  static constexpr int kN = 128 * NM;
-  static constexpr int kRawDyBytes = kWgBatch * kN * 4;
-  static constexpr int kRawXBytes = kWgBatch * LDX * 4;
-  static constexpr int kRawBytes = kRawDyBytes + kRawXBytes;
-  static constexpr int kAPlane = 2 * 128 * 16;               // one out-feature block, one of {hi, lo}: [k8 2][128][8]
-  static constexpr int kBPlane = 2 * KP * 16;                // one of {hi, lo} of X^T: [k8 2][KP][8]
-  static constexpr int kPlanesBytes = 2 * NM * kAPlane + 2 * kBPlane;
-  static constexpr int kRingBytes = kWgRawStages * kRawBytes + kWgPlaneBufs * kPlanesBytes;
-  static constexpr int kOutLd = KP + 4;
-  static constexpr int kOutBytes = 128 * kOutLd * 4;         // epilogue staging (one block at a time), aliases the ring
-  static constexpr int kSmemBytes = (kRingBytes > kOutBytes ? kRingBytes : kOutBytes) + 1024;
-  static constexpr int kTmemColsRaw = NM * KP;
-  static constexpr int kTmemCols = kTmemColsRaw < 32 ? 32 : kTmemColsRaw;
-  static_assert((kTmemCols & (kTmemCols - 1)) == 0 && kTmemCols <= 512, "TMEM columns");
-  static_assert(kSmemBytes <= 227 * 1024, "shared memory");
+template <int FB>
+struct WtGeo {
+  static constexpr int kDyPlane = 128 * 32 * 2;        // one 128-feature x 32-point bf16 plane
+  static constexpr int kXPlane = FB * 32 * 2;
+  static constexpr int kBufBytes = 2 * kDyPlane + 2 * kXPlane;   // dY hi, dY lo, X hi, X lo
+  static constexpr int kSmemBytes = 2 * kBufBytes + 1024;
 };
 
 struct WgradTcArgs {
-  const float* dY;                   // (P, N) contiguous rows
-  const float* X;                    // (P, LDX) contiguous rows
-  int K;                             // valid columns of X (<= KP)
-  float* dW; int ldw; int col_off;   // dW (N, ldw): the block lands at columns [col_off, col_off + K)
+  const float* dY; int N;
+  const float* X; int ldx; int K;
+  float* dW; int ldw; int col_off;
   float* db;                         // nullable
-  uint32_t* x_pos_bits;              // nullable, KP = 256 only: (P, 8) words, bit c of word w = [X[p][32 w + c] > 0]
+  uint32_t* x_pos_bits;              // nullable, K = 256 only: (P, 8) words, bit c of word w = [X[p][32 w + c] > 0]
   long long P;
-  long long rows_per_split;          // multiple of kWgBatch
+  long long n_tiles, tiles_per_cta;
 };
 
-// 8 consecutive points of one feature column -> one 16-byte row of the hi plane and of the lo plane
-__device__ __forceinline__ void split8_store(const float (&v)[8], unsigned char* hi_dst, unsigned char* lo_dst) {
+template <int FB>
+__device__ __forceinline__ void wgmma_mn_bf16(float (&d)[FB / 2], uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (FB == 256) wgmma_m64n256_bf16_mn(d, a, b, acc);
+  else if constexpr (FB == 64) wgmma_m64n64_bf16_mn(d, a, b, acc);
+  else wgmma_m64n32_bf16_mn(d, a, b, acc);
+}
+
+// 8 fp32 values -> a 16-byte bf16 hi cell and the matching lo cell
+__device__ __forceinline__ void split8_bf16(const float (&v)[8], uint4& hi, uint4& lo) {
   uint32_t h[4], l[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    const __nv_bfloat162 hh = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-    h[j] = *reinterpret_cast<const uint32_t*>(&hh);
-    const float b0 = __uint_as_float(h[j] << 16), b1 = __uint_as_float(h[j] & 0xffff0000u);
-    const __nv_bfloat162 ll = __floats2bfloat162_rn(v[2 * j] - b0, v[2 * j + 1] - b1);
-    l[j] = *reinterpret_cast<const uint32_t*>(&ll);
+    const __nv_bfloat162 b = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
+    h[j] = *reinterpret_cast<const uint32_t*>(&b);
+    const __nv_bfloat162 r = __floats2bfloat162_rn(v[2 * j] - __low2float(b), v[2 * j + 1] - __high2float(b));
+    l[j] = *reinterpret_cast<const uint32_t*>(&r);
   }
-  *reinterpret_cast<uint4*>(hi_dst) = make_uint4(h[0], h[1], h[2], h[3]);
-  *reinterpret_cast<uint4*>(lo_dst) = make_uint4(l[0], l[1], l[2], l[3]);
+  hi = make_uint4(h[0], h[1], h[2], h[3]);
+  lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
-template <int KP, int NM, int LDX>
-__global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(WgradTcArgs a) {
-  using G = WgGeo<KP, NM, LDX>;
-  constexpr int kN = G::kN;
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  unsigned char* ring = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  unsigned char* planes0 = ring + kWgRawStages * G::kRawBytes;
-  __shared__ uint64_t raw_full[kWgRawStages], raw_empty[kWgRawStages], pl_full[kWgPlaneBufs], pl_empty[kWgPlaneBufs], d_full;
-  __shared__ uint32_t tmem_base_s;
+template <int FB>
+__global__ void __launch_bounds__(kWtThreads, 1) wgrad_tc_kernel(WgradTcArgs a) {
+  using G = WtGeo<FB>;
+  extern __shared__ unsigned char smem_raw[];
+  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  __shared__ uint8_t pos[32][FB / 8];             // [X > 0] of one tile, one byte per 8-feature cell
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const long long r_begin = (long long)blockIdx.x * a.rows_per_split;
-  const long long r_end = r_begin + a.rows_per_split < a.P ? r_begin + a.rows_per_split : a.P;
-  const int n_batches = r_end > r_begin ? (int)((r_end - r_begin + kWgBatch - 1) / kWgBatch) : 0;
+  const int mb = blockIdx.y;
+  const long long t_begin = (long long)blockIdx.x * a.tiles_per_cta;
+  const long long t_end = t_begin + a.tiles_per_cta < a.n_tiles ? t_begin + a.tiles_per_cta : a.n_tiles;
+  const int n_my = t_end > t_begin ? (int)(t_end - t_begin) : 0;
+  if (n_my == 0) return;
+  const bool emit_bits = a.x_pos_bits != nullptr && mb == 0;
+  const int wgi = warp >> 2, wq = warp & 3, g = lane >> 2, tq = lane & 3;
 
-  if (tid == 0) {
-    for (int i = 0; i < kWgRawStages; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], kWgConvWarps * 32); }
-    for (int i = 0; i < kWgPlaneBufs; ++i) { mbar_init(&pl_full[i], kWgConvWarps * 32); mbar_init(&pl_empty[i], 1); }
-    mbar_init(&d_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == kWgMmaWarp) tmem_alloc<G::kTmemCols>(&tmem_base_s);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tbase = tmem_base_s;
+  float bs[8];                                     // bias partial sums of feature group tid % 16
+#pragma unroll
+  for (int j = 0; j < 8; ++j) bs[j] = 0.f;
+  float acc[FB / 2];
+#pragma unroll
+  for (int i = 0; i < FB / 2; ++i) acc[i] = 0.f;
 
-  if (warp == kWgLoadWarp) {
-    // ======================= producer: HBM -> raw fp32 ring (bulk copies) =======================
-    if (elect_one()) {
-      for (int bi = 0; bi < n_batches; ++bi) {
-        const int rs = bi % kWgRawStages;
-        mbar_wait(&raw_empty[rs], ((bi / kWgRawStages) & 1) ^ 1);
-        const long long p0 = r_begin + (long long)bi * kWgBatch;
-        const uint32_t rows = (uint32_t)(r_end - p0 < kWgBatch ? r_end - p0 : kWgBatch);
-        unsigned char* dst = ring + (size_t)rs * G::kRawBytes;
-        mbar_arrive_expect_tx(&raw_full[rs], rows * (uint32_t)(kN * 4 + LDX * 4));
-        bulk_g2s(dst, a.dY + (size_t)p0 * kN, rows * kN * 4, &raw_full[rs]);
-        bulk_g2s(dst + G::kRawDyBytes, a.X + (size_t)p0 * LDX, rows * LDX * 4, &raw_full[rs]);
+  for (int i = 0; i < n_my; ++i) {
+    // every thread of both warpgroups has passed the wait that retired tile i - 2, the last reader of this buffer
+    // (and the previous tile's sign bits have been read out of pos[])
+    __syncthreads();
+    unsigned char* buf = smem + (size_t)(i & 1) * G::kBufBytes;
+    unsigned char* dy_hi = buf;
+    unsigned char* dy_lo = buf + G::kDyPlane;
+    unsigned char* x_hi = buf + 2 * G::kDyPlane;
+    unsigned char* x_lo = x_hi + G::kXPlane;
+    const long long p0 = (t_begin + i) * 32;
+    // ---- dY block: 16 feature groups x 32 points, two cells per thread (same group: the bias sums stay in registers)
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const int e = tid + c * kWtThreads, grp = e & 15, p = e >> 4;
+      const long long pt = p0 + p;
+      float v[8];
+      if (pt < a.P) {
+        const float4* src = reinterpret_cast<const float4*>(a.dY + pt * a.N + mb * 128 + grp * 8);
+        const float4 u0 = __ldg(src), u1 = __ldg(src + 1);
+        v[0] = u0.x; v[1] = u0.y; v[2] = u0.z; v[3] = u0.w; v[4] = u1.x; v[5] = u1.y; v[6] = u1.z; v[7] = u1.w;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = 0.f;
       }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) bs[j] += v[j];
+      uint4 h, l;
+      split8_bf16(v, h, l);
+      *reinterpret_cast<uint4*>(dy_hi + grp * 512 + p * 16) = h;
+      *reinterpret_cast<uint4*>(dy_lo + grp * 512 + p * 16) = l;
     }
-    __syncwarp();
-  } else if (warp == kWgMmaWarp) {
-    // ======================= MMA issuer =======================
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc(kFmtBF16, 128, KP);
-      for (int bi = 0; bi < n_batches; ++bi) {
-        const int pb = bi % kWgPlaneBufs;
-        mbar_wait(&pl_full[pb], (bi / kWgPlaneBufs) & 1);
-        tc_fence_after();
-        const uint32_t base = smem_u32(planes0 + (size_t)pb * G::kPlanesBytes);
-        const uint32_t b_base = base + 2 * NM * G::kAPlane;
-        const uint64_t b_hi = make_smem_desc(b_base, KP * 16, 128);
-        const uint64_t b_lo = make_smem_desc(b_base + G::kBPlane, KP * 16, 128);
+    // ---- X tile: FB / 8 feature groups x 32 points
+    for (int e = tid; e < (FB / 8) * 32; e += kWtThreads) {
+      const int grp = e % (FB / 8), p = e / (FB / 8);
+      const long long pt = p0 + p;
+      float v[8];
 #pragma unroll
-        for (int mb = 0; mb < NM; ++mb) {
-          const uint64_t a_hi = make_smem_desc(base + mb * G::kAPlane, 128 * 16, 128);
-          const uint64_t a_lo = make_smem_desc(base + (NM + mb) * G::kAPlane, 128 * 16, 128);
-          const uint32_t d = tbase + mb * KP;
-          mma_ss(d, a_hi, b_hi, idesc, bi > 0 ? 1u : 0u);
-          mma_ss(d, a_lo, b_hi, idesc, 1u);
-          mma_ss(d, a_hi, b_lo, idesc, 1u);
-        }
-        mma_commit(&pl_empty[pb]);
-      }
-      mma_commit(&d_full);
-    }
-    __syncwarp();
-  } else {
-    // ======================= converters: raw fp32 tile -> bf16 hi | lo planes, points-major =====
-    // group = (feature, k8 block): 8 consecutive points of one feature.  dY^T has kN x 2 groups per
-    // batch, X^T has KP x 2; group g of a thread = index tid + 256 g -> feature idx % F, k8 idx / F.
-    constexpr int kGa = (kN * 2) / 256, kGb = (KP * 2 + 255) / 256;
-    float bias_acc[kGa];
-#pragma unroll
-    for (int g = 0; g < kGa; ++g) bias_acc[g] = 0.f;
-    for (int bi = 0; bi < n_batches; ++bi) {
-      const int rs = bi % kWgRawStages, pb = bi % kWgPlaneBufs;
-      const long long p0 = r_begin + (long long)bi * kWgBatch;
-      const int rows = (int)(r_end - p0 < kWgBatch ? r_end - p0 : kWgBatch);
-      mbar_wait(&raw_full[rs], (bi / kWgRawStages) & 1);
-      const float* raw_dy = reinterpret_cast<const float*>(ring + (size_t)rs * G::kRawBytes);
-      const float* raw_x = reinterpret_cast<const float*>(ring + (size_t)rs * G::kRawBytes + G::kRawDyBytes);
-      float va[kGa][8], vb[kGb][8];
-#pragma unroll
-      for (int g = 0; g < kGa; ++g) {
-        const int idx = tid + 256 * g, f = idx % kN, j = idx / kN;
-#pragma unroll
-        for (int r = 0; r < 8; ++r) va[g][r] = (j * 8 + r < rows) ? raw_dy[(j * 8 + r) * kN + f] : 0.f;
-      }
-#pragma unroll
-      for (int g = 0; g < kGb; ++g) {
-        const int idx = tid + 256 * g, f = idx % KP, j = idx / KP;
-#pragma unroll
-        for (int r = 0; r < 8; ++r) vb[g][r] = (j < 2 && j * 8 + r < rows && f < a.K) ? raw_x[(j * 8 + r) * LDX + f] : 0.f;
-      }
-      mbar_arrive(&raw_empty[rs]);                 // the raw tile is in registers
-      mbar_wait(&pl_empty[pb], ((bi / kWgPlaneBufs) & 1) ^ 1);
-      unsigned char* pl = planes0 + (size_t)pb * G::kPlanesBytes;
-#pragma unroll
-      for (int g = 0; g < kGa; ++g) {
-        const int idx = tid + 256 * g, f = idx % kN, j = idx / kN;
-#pragma unroll
-        for (int r = 0; r < 8; ++r) bias_acc[g] += va[g][r];
-        const int mb = f >> 7, off = j * (128 * 16) + (f & 127) * 16;
-        split8_store(va[g], pl + mb * G::kAPlane + off, pl + (NM + mb) * G::kAPlane + off);
-      }
-#pragma unroll
-      for (int g = 0; g < kGb; ++g) {
-        const int idx = tid + 256 * g, f = idx % KP, j = idx / KP;
-        if (j < 2) {
-          const int off = j * (KP * 16) + f * 16;
-          split8_store(vb[g], pl + 2 * NM * G::kAPlane + off, pl + 2 * NM * G::kAPlane + G::kBPlane + off);
-        }
-        if (KP == 256 && a.x_pos_bits != nullptr) {
-          // the ReLU mask the following dgrad needs, as a by-product: a warp holds 32 consecutive features
-          // of the same 8 points, so one ballot per point is that point's mask word
-          uint32_t mine = 0;
-#pragma unroll
-          for (int r = 0; r < 8; ++r) {
-            const uint32_t w = __ballot_sync(0xffffffffu, vb[g][r] > 0.f);
-            if (lane == r) mine = w;
-          }
-          if (lane < 8 && j * 8 + lane < rows) a.x_pos_bits[(p0 + j * 8 + lane) * 8 + (f >> 5)] = mine;
-        }
-      }
-      fence_proxy_async_smem();     // generic-proxy smem writes -> visible to tcgen05.mma
-      mbar_arrive(&pl_full[pb]);
-    }
-    if (a.db != nullptr && n_batches > 0) {
-#pragma unroll
-      for (int g = 0; g < kGa; ++g) atomicAdd(a.db + (tid + 256 * g) % kN, bias_acc[g]);
-    }
-
-    // ======================= epilogue: TMEM -> smem -> atomics, one out-feature block at a time ==
-    if (n_batches > 0) {
-      mbar_wait(&d_full, 0);
-      tc_fence_after();
-      float* out = reinterpret_cast<float*>(ring);       // [128][KP + 4]; every copy and MMA has retired
-      constexpr int kLd = G::kOutLd;
-#pragma unroll 1
-      for (int mb = 0; mb < NM; ++mb) {
-        if (warp < 4) {
-          const int row = warp * 32 + lane;
-#pragma unroll 1
-          for (int c0 = 0; c0 < KP; c0 += 32) {
-            uint32_t v[32];
-            tmem_ld32(tbase + ((uint32_t)(warp * 32) << 16) + mb * KP + c0, v);
-            tmem_wait_ld();
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              *reinterpret_cast<float4*>(out + row * kLd + c0 + j) =
-                  make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-          }
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kWgConvWarps * 32) : "memory");
-        if (KP % 4 == 0 && a.K == KP && ((a.ldw | a.col_off) & 3) == 0 && (reinterpret_cast<uintptr_t>(a.dW) & 15) == 0) {
-          // 16-byte vector reductions (red.global.add.v4.f32): a quarter of the L2 atomic operations
-          for (int e = tid; e < 128 * (KP / 4); e += kWgConvWarps * 32) {
-            const int m = e / (KP / 4), k = (e - m * (KP / 4)) * 4;
-            const float4 v = *reinterpret_cast<const float4*>(out + m * kLd + k);
-            float* dst = a.dW + (size_t)(mb * 128 + m) * a.ldw + a.col_off + k;
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-                         : "memory");
-          }
+      for (int j = 0; j < 8; ++j) v[j] = 0.f;
+      if (pt < a.P) {
+        const float* src = a.X + pt * a.ldx + grp * 8;
+        if (grp * 8 + 8 <= a.K) {
+          const float4 u0 = __ldg(reinterpret_cast<const float4*>(src)), u1 = __ldg(reinterpret_cast<const float4*>(src) + 1);
+          v[0] = u0.x; v[1] = u0.y; v[2] = u0.z; v[3] = u0.w; v[4] = u1.x; v[5] = u1.y; v[6] = u1.z; v[7] = u1.w;
         } else {
-          for (int e = tid; e < 128 * KP; e += kWgConvWarps * 32) {
-            const int m = e / KP, k = e - m * KP;
-            if (k < a.K) atomicAdd(a.dW + (size_t)(mb * 128 + m) * a.ldw + a.col_off + k, out[m * kLd + k]);
-          }
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[j] = grp * 8 + j < a.K ? __ldg(src + j) : 0.f;
         }
-        asm volatile("bar.sync 1, %0;" ::"n"(kWgConvWarps * 32) : "memory");
       }
+      if (FB == 256 && emit_bits) {
+        uint32_t b = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) b |= (v[j] > 0.f ? 1u : 0u) << j;
+        pos[p][grp] = (uint8_t)b;
+      }
+      uint4 h, l;
+      split8_bf16(v, h, l);
+      *reinterpret_cast<uint4*>(x_hi + grp * 512 + p * 16) = h;
+      *reinterpret_cast<uint4*>(x_lo + grp * 512 + p * 16) = l;
+    }
+    fence_proxy_async_smem();     // generic-proxy smem writes -> visible to the wgmmas
+    __syncthreads();
+    if (FB == 256 && emit_bits) {
+      // thread = (point tid / 8, word tid % 8): four bytes of the tile's sign bits -> one word
+      const int p = tid >> 3, w = tid & 7;
+      const long long pt = p0 + p;
+      if (pt < a.P)
+        a.x_pos_bits[pt * 8 + w] = (uint32_t)pos[p][4 * w] | ((uint32_t)pos[p][4 * w + 1] << 8) |
+                                   ((uint32_t)pos[p][4 * w + 2] << 16) | ((uint32_t)pos[p][4 * w + 3] << 24);
+    }
+    wgmma_fence();
+    const uint32_t ah = smem_u32(dy_hi) + wgi * (8 * 512), al = smem_u32(dy_lo) + wgi * (8 * 512);
+    const uint32_t bh = smem_u32(x_hi), bl = smem_u32(x_lo);
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+      const uint64_t dah = make_smem_desc(ah + ks * 256, 128, 512), dal = make_smem_desc(al + ks * 256, 128, 512);
+      const uint64_t dbh = make_smem_desc(bh + ks * 256, 128, 512), dbl = make_smem_desc(bl + ks * 256, 128, 512);
+      wgmma_mn_bf16<FB>(acc, dah, dbh, (i > 0 || ks > 0) ? 1u : 0u);
+      wgmma_mn_bf16<FB>(acc, dal, dbh, 1u);
+      wgmma_mn_bf16<FB>(acc, dah, dbl, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();              // tile i - 1 has retired
+  }
+  wgmma_wait<0>();
+
+  if (a.db != nullptr) {
+    // threads t and t ^ 16 of a warp share a feature group; then one atomic per warp and feature
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float v = bs[j] + __shfl_xor_sync(0xffffffffu, bs[j], 16);
+      if (lane < 16) atomicAdd(a.db + mb * 128 + (tid & 15) * 8 + j, v);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWgMmaWarp) tmem_dealloc<G::kTmemCols>(tbase);
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int m = mb * 128 + wgi * 64 + wq * 16 + g + 8 * rr;
+    float* dst = a.dW + (size_t)m * a.ldw + a.col_off;
+#pragma unroll
+    for (int j = 0; j < FB / 8; ++j) {
+      const int k = 8 * j + 2 * tq;
+      if (k < a.K) red_add_pair(dst + k, acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1], k + 1 < a.K);
+    }
+  }
 }
 
-int wg_sms() { return sm_count(); }
-
-template <int KP, int NM, int LDX>
+template <int FB>
 int launch_wgrad_tc(WgradTcArgs a, cudaStream_t st) {
-  using G = WgGeo<KP, NM, LDX>;
+  using G = WtGeo<FB>;
   static SmemOptIn optin;
-  if (int rc = ensure_smem(wgrad_tc_kernel<KP, NM, LDX>, optin, G::kSmemBytes, "wgrad_tc")) return rc;
-  int splits = wg_sms();
-  long long rows = (a.P + splits - 1) / splits;
-  rows = (rows + kWgBatch - 1) / kWgBatch * kWgBatch;
-  splits = (int)((a.P + rows - 1) / rows);
-  a.rows_per_split = rows;
-  wgrad_tc_kernel<KP, NM, LDX><<<splits, kWgThreads, G::kSmemBytes, st>>>(a);
+  if (int rc = ensure_smem(wgrad_tc_kernel<FB>, optin, G::kSmemBytes, "wgrad_tc")) return rc;
+  const int blocks = a.N / 128;
+  long long ctas = (sm_count() + blocks - 1) / blocks;
+  if (ctas > a.n_tiles) ctas = a.n_tiles;
+  a.tiles_per_cta = (a.n_tiles + ctas - 1) / ctas;
+  ctas = (a.n_tiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
+  wgrad_tc_kernel<FB><<<dim3((unsigned)ctas, blocks), kWtThreads, G::kSmemBytes, st>>>(a);
   return check_launch("wgrad_tc_kernel");
 }
 
 }  // namespace
 
-// run_wgrad (field_bwd.cu) on tensor cores: same accumulate-into semantics; optionally also emits the
-// sign bits of X (the ReLU mask of the layer's input) for the dgrad that follows.  dY is (P, N) with
-// N = 128 or 256, X is (P, ldx) with (K, ldx) one of (256, 256), (63, 64), (27, 32).
 int run_wgrad_tc(const float* dY, int N, const float* X, int ldx, int K, float* dW, int ldw, int col_off, float* db,
                  uint32_t* x_pos_bits, long long P, cudaStream_t st) {
   if (P == 0) return SNB_OK;
   if (x_pos_bits != nullptr && K != 256) return fail(SNB_ERR_INVALID, "run_wgrad_tc: mask bits need K = 256");
-  if ((reinterpret_cast<uintptr_t>(dY) | reinterpret_cast<uintptr_t>(X)) & 15)
+  if (((reinterpret_cast<uintptr_t>(dY) | reinterpret_cast<uintptr_t>(X)) & 15) != 0)
     return fail(SNB_ERR_INVALID, "run_wgrad_tc: dY and X must be 16-byte aligned");
-  WgradTcArgs a{dY, X, K, dW, ldw, col_off, db, x_pos_bits, P, 0};
-  if (N == 256 && ldx == 256 && K == 256) return launch_wgrad_tc<256, 2, 256>(a, st);
-  if (N == 128 && ldx == 256 && K == 256) return launch_wgrad_tc<256, 1, 256>(a, st);
-  if (N == 256 && ldx == 64 && K <= 64) return launch_wgrad_tc<64, 2, 64>(a, st);
-  if (N == 128 && ldx == 32 && K <= 32) return launch_wgrad_tc<32, 1, 32>(a, st);
+  WgradTcArgs a{dY, N, X, ldx, K, dW, ldw, col_off, db, x_pos_bits, P, (P + 31) / 32, 0};
+  if (N != 256 && N != 128) return fail(SNB_ERR_INVALID, "run_wgrad_tc: unsupported out features N=%d", N);
+  if (ldx == 256 && K == 256) return launch_wgrad_tc<256>(a, st);
+  if (ldx == 64 && K <= 64) return launch_wgrad_tc<64>(a, st);
+  if (ldx == 32 && K <= 32) return launch_wgrad_tc<32>(a, st);
   return fail(SNB_ERR_INVALID, "run_wgrad_tc: unsupported shape N=%d K=%d ldx=%d", N, K, ldx);
 }
 

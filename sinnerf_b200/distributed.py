@@ -51,8 +51,7 @@ class PixelGather:
     """Double-buffered, asynchronous all-gather of rendered pixel slabs for back-to-back frames.
 
     A blocking `all_gather_into_tensor` after every frame makes the collective a per-step barrier: every rank
-    waits for the slowest one each step (measured in round 1 on 8 power-capped B200s: 61.9 -> 64.4 ms per step
-    while the render kernel itself moved 41.3 -> 41.7 ms).  Here gather k runs on NCCL's own stream while the
+    waits for the slowest one each step.  Here gather k runs on NCCL's own stream while the
     ranks already render frame k + 1; a rank only waits when it is TWO frames ahead (its buffer k - 2 is still
     in flight).  `wait_all()` before reading the last results / stopping a clock."""
 

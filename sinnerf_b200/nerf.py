@@ -1,5 +1,5 @@
 """`Embedding` and `NeRF` with the reference's constructor signatures, attributes and state-dict
-(reference models/nerf.py:7-41, :46-148), executing on libsinnerf_b200's sm_100a kernels.
+(reference models/nerf.py:7-41, :46-148), executing on libsinnerf_b200's sm_90a kernels.
 
 The modules are parameter containers: `nn.Linear` leaves with the reference's names
 (`xyz_encoding_{1..8}.0.{weight,bias}`, `xyz_encoding_final.*`, `dir_encoding.0.*`, `sigma.*`,
@@ -22,7 +22,7 @@ class ShiftedSoftplus(nn.Module):
     """Marker for reference models/activations.py:54-71; evaluated inside the fused kernels."""
 
     def forward(self, x):  # pragma: no cover - never on the hot path
-        raise RuntimeError("activation is fused into the sm_100a field kernel; call NeRF.forward")
+        raise RuntimeError("activation is fused into the sm_90a field kernel; call NeRF.forward")
 
 
 class WidenedSigmoid(ShiftedSoftplus):

@@ -1,6 +1,6 @@
 """Fused Adam for the NeRF MLPs (SURVEY 8f-4): `torch.optim.Adam` as the reference's `get_optimizer` configures
 it (reference utils/__init__.py:10-31: lr, eps = 1e-8, weight_decay) with the whole update of one model --
-all 24 tensors -- in ONE sm_100a kernel, followed on the same stream by the re-pack of the weight image the
+all 24 tensors -- in ONE sm_90a kernel, followed on the same stream by the re-pack of the weight image the
 field kernels stream, so the next forward finds it up to date (and stamped clean) without re-packing.
 
 `FusedAdam` is a `torch.optim.Optimizer`: `param_groups[0]['lr']` is honoured every step, so the reference's

@@ -1,6 +1,6 @@
 """`render_rays`, `sample_pdf`, `eval_points` with the reference's signatures
 (reference models/rendering.py:15-61, :64-123, :126-335), executed by libsinnerf_b200's
-sm_100a kernels through the C ABI in include/sinnerf_b200.h.
+sm_90a kernels through the C ABI in include/sinnerf_b200.h.
 
 Host side only: argument checks, output allocation from PyTorch's caching allocator, the
 reference's random draws (same shapes, same order, same torch generator, so a seeded run

@@ -23,7 +23,13 @@ def room_params(which):
     """'coarse' | 'fine' -> {state-dict key: fp32 tensor} of the reference's trained checkpoint."""
     global _room
     if _room is None:
-        _room = load_npz("room_weights.npz")
+        # stored in parts of < 1 MB each: room_weights_0.npz, room_weights_1.npz, ...
+        _room = {}
+        i = 0
+        while os.path.exists(os.path.join(GOLDEN, f"room_weights_{i}.npz")):
+            _room.update(load_npz(f"room_weights_{i}.npz"))
+            i += 1
+        assert _room, "tests/golden/room_weights_*.npz missing"
     pre = which + "/"
     return {k[len(pre):]: torch.from_numpy(v.copy()) for k, v in _room.items() if k.startswith(pre)}
 

@@ -11,10 +11,13 @@ every stage of the hot path.  Nothing here is used at run time by the product;
 tests compare (a) the oracle and (b) the CUDA path against these files.
 
 Outputs (tests/golden/):
-  room_weights.npz   the reference's trained checkpoint ckpts/room.ckpt re-saved
-                     as plain arrays (realistic weight statistics; SURVEY.md 2 #15)
+  room_weights_*.npz the reference's trained checkpoint ckpts/room.ckpt re-saved
+                     as plain arrays, in parts of < 1 MB (realistic weight statistics; SURVEY.md 2 #15)
   stages.npz         Embedding / NeRF.forward / sample_pdf / activations goldens
   render_*.npz       whole render_rays cases (rays, config, RNG tensors, outputs)
+  reference_live.npz the reference's outputs / gradients on the randomised cases of
+                     tests/test_oracle_vs_reference_live.py (gradients: a seeded sample
+                     of each tensor plus its norm)
 """
 import os
 import sys
@@ -181,6 +184,85 @@ def c1_full():
                 n_importance=0, white_back=False)
 
 
+ROOM_PART_BYTES = 900 * 1024   # raw bytes per part: the .npz (header + arrays) stays below 1 MB
+
+
+def save_room_parts(room):
+    """room_weights_{0,1,...}.npz: the arrays in key order, a part closed before a tensor would take it past
+    ROOM_PART_BYTES (tests/_common.py room_params merges them)."""
+    for f in os.listdir(HERE):
+        if f.startswith("room_weights_") and f.endswith(".npz"):
+            os.remove(os.path.join(HERE, f))
+    part, size, i = {}, 0, 0
+    for k in sorted(room):
+        if part and size + room[k].nbytes > ROOM_PART_BYTES:
+            np.savez_compressed(os.path.join(HERE, f"room_weights_{i}.npz"), **part)
+            part, size, i = {}, 0, i + 1
+        part[k] = room[k]
+        size += room[k].nbytes
+    if part:
+        np.savez_compressed(os.path.join(HERE, f"room_weights_{i}.npz"), **part)
+    for j in range(i + 1):
+        assert os.path.getsize(os.path.join(HERE, f"room_weights_{j}.npz")) < 1_000_000
+
+
+def live_golden():
+    """What tests/test_oracle_vs_reference_live.py compares the oracle against, computed by the reference."""
+    from tests.test_oracle_vs_reference_live import CASES, GRAD_SAMPLE, grad_case_inputs, grad_sample_index
+    out = {}
+
+    def models_of(params):
+        ms = []
+        for p in params:
+            m = NeRF(use_new_activation=True)
+            m.load_state_dict(p)
+            ms.append(m.eval())
+        return ms
+
+    for i, (shape, n, S, Ni, use_disp, perturb, noise_std, white_back, seed) in enumerate(CASES):
+        rays = synthetic.random_rays(shape, n, seed=seed)
+        models = models_of([default_init_params(10 + seed), default_init_params(20 + seed)])
+        emb = [Embedding(3, 10), Embedding(3, 4)]
+        with torch.no_grad():
+            torch.manual_seed(100 + seed)
+            want = render_rays(models, emb, rays, S, use_disp, perturb, noise_std, Ni, 1024, white_back, test_time=False)
+        for k, v in want.items():
+            out[f"case{i}/{k}"] = np_(v)
+    rays = synthetic.random_rays("lego", 12, seed=9)
+    models = models_of([default_init_params(1), default_init_params(2)])
+    with torch.no_grad():
+        want = render_rays(models, [Embedding(3, 10), Embedding(3, 4)], rays, 64, False, 0, 0, 64, 1024, True, test_time=True)
+    for k, v in want.items():
+        out[f"testtime/{k}"] = np_(v)
+    for seed in (0, 1, 2):
+        g = torch.Generator().manual_seed(seed)
+        n, m, ni = 19, 23 + seed, 31
+        bins = torch.sort(torch.rand(n, m + 1, generator=g) * 4 + 2, dim=-1).values
+        w = torch.rand(n, m, generator=g) ** 3
+        w[0] = 0.0
+        out[f"pdf{seed}"] = np_(sample_pdf(bins, w, ni, det=True))
+    rays, pc, pf, proj_seed = grad_case_inputs()
+    models = models_of([pc, pf])
+    for m in models:
+        m.train()
+    torch.manual_seed(77)
+    want = render_rays(models, [Embedding(3, 10), Embedding(3, 4)], rays, 32, False, 1.0, 1.0, 24, 1024, False, test_time=False)
+    g = torch.Generator().manual_seed(proj_seed)
+    proj = {k: torch.randn(v.shape, generator=g) for k, v in want.items()}
+    sum((want[k] * proj[k]).sum() for k in want).backward()
+    for k, v in proj.items():
+        out[f"proj/{k}"] = np_(v)
+    for tag, model in (("coarse", models[0]), ("fine", models[1])):
+        for k, v in model.named_parameters():
+            if v.grad is None:
+                continue
+            out[f"grad/{tag}/{k}/norm"] = np.float64(float(v.grad.double().norm()))
+            out[f"grad/{tag}/{k}/sample"] = np_(v.grad.reshape(-1)[grad_sample_index(v.numel(), GRAD_SAMPLE)])
+    path = os.path.join(HERE, "reference_live.npz")
+    np.savez_compressed(path, **out)
+    print("wrote", path, len(out), "arrays")
+
+
 def main():
     if "--only-c1-full" in sys.argv:
         c1_full()
@@ -192,7 +274,7 @@ def main():
     if "--grad-only" in sys.argv:
         grad_golden(room)
         return
-    np.savez_compressed(os.path.join(HERE, "room_weights.npz"), **room)
+    save_room_parts(room)
     print("room_weights:", len(room), "tensors")
 
     # ---------------- stage goldens ----------------
@@ -266,6 +348,7 @@ def main():
     grad_golden(room)
     rays_golden()
     c1_full()
+    live_golden()
 
 
 if __name__ == "__main__":

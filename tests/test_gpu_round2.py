@@ -33,7 +33,7 @@ def embeddings():
 @pytest.mark.parametrize("shape,white_back", [("lego", True), ("dtu", True)])
 def test_full_frame_subset_matches_oracle(shape, white_back):
     """BASELINE configs[1] (400x400 = 160 000 rays) and configs[3] (640x512 = 327 680 rays) rendered IN FULL by the
-    persistent 148-CTA kernels; a seeded 2 048-ray subset of the result against the CPU oracle at the SURVEY 8c
+    persistent one-CTA-per-SM kernels; a seeded 2 048-ray subset of the result against the CPU oracle at the SURVEY 8c
     tolerances (tile tails / slot wrap-around only exist at this size).  Also pins how many fine-pass depths of a
     full frame land in a different bin than the oracle's (the cdf is a warp scan here, a serial cumsum there)."""
     from sinnerf_b200 import synthetic
@@ -458,7 +458,7 @@ def test_fp16_training_storage_matches_fp32_storage_and_oracle(weights, n_rays, 
                 worst_o, worst_o32 = max(worst_o, e16), max(worst_o32, e32)
                 # Trained weights: the 1e-3 bar of SURVEY 8c against the oracle.  Default-init weights leave ReLU
                 # pre-activations within rounding of zero that flip between ANY two implementations (all-fp32 ones too:
-                # profiles/r01_grad_error.txt, the smoke test's note) -- at 1 500 rays the first layer's gradient of the
+                # the smoke test's note) -- at 1 500 rays the first layer's gradient of the
                 # fp32-STORAGE kernels already differs from the oracle's by ~1.4e-3 with or without training noise
                 # (measured on HEAD 5fa9a95 and on this build alike), so there the 16-bit path is held to the
                 # fp32-storage kernels (1e-3, above) and, against the oracle, to no more than 1.25x their deviation.

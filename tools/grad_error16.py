@@ -21,9 +21,8 @@ n = int(sys.argv[1]) if len(sys.argv) > 1 else 256
 which = sys.argv[2] if len(sys.argv) > 2 else "seed"
 dev = torch.device("cuda:0")
 if which == "room":
-    z = np.load(os.path.join(os.path.dirname(__file__), "..", "tests", "golden", "room_weights.npz"))
-    pc = {k[7:]: torch.from_numpy(z[k].copy()) for k in z.files if k.startswith("coarse/")}
-    pf = {k[5:]: torch.from_numpy(z[k].copy()) for k in z.files if k.startswith("fine/")}
+    from tests._common import room_params
+    pc, pf = room_params("coarse"), room_params("fine")
     rays = synthetic.random_rays("llff", n, seed=3)
 else:
     pc, pf = orc.default_init_params(0), orc.default_init_params(1)

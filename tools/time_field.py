@@ -55,8 +55,9 @@ for _ in range(args.iters):
     ts.append(e0.elapsed_time(e1))
 ms = min(ts)
 flops = 2 * (982528 // 2 if args.sigma_only else 593408) * n * S
-print(f"precision={args.precision} debug={os.environ.get('SNB_TC_DEBUG', '0')} rays={n} S={S} "
+sms = torch.cuda.get_device_properties(0).multi_processor_count
+print(f"precision={args.precision} rays={n} S={S} "
       f"ms={ms:.3f} (median {sorted(ts)[len(ts) // 2]:.3f})  {flops / ms / 1e9:.1f} TFLOP/s algorithmic  "
-      f"{n * S / 128 / 148 :.0f} tiles/SM  {ms * 1e3 / (n * S / 128 / 148):.2f} us/tile")
+      f"{n * S / 128 / sms :.0f} tiles/SM  {ms * 1e3 / (n * S / 128 / sms):.2f} us/tile")
 if args.dump:
     torch.save(raw.cpu(), args.dump)
