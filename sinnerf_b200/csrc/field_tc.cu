@@ -4,22 +4,27 @@
 // [r,g,b,sigma] out; reference models/rendering.py:184-212,284-285 + models/nerf.py:24-41,
 // 105-148), but every 256-wide layer is a chain of wgmma.mma_async instructions:
 //
-//   * persistent CTAs of two warpgroups; a CTA works on 128-point tiles,
-//     each warpgroup owns 64 of the rows (wgmma M = 64) and both share one weight stream, so every
-//     weight byte a CTA ingests from L2 feeds 128 points;
+//   * persistent CTAs of two consumer warpgroups and one producer warpgroup; a CTA works on 128-point
+//     tiles, each consumer warpgroup owns 64 of the rows (wgmma M = 64) and both share one weight stream,
+//     so every weight byte a CTA ingests from L2 feeds 128 points; setmaxnreg moves the producer's
+//     registers to the consumers (24 / 240 per thread);
 //   * a layer's whole 64 x 256 fp32 accumulator lives in registers (two N = 128 halves, 128 registers
 //     per thread); the epilogue adds the bias, applies ReLU, splits the value into a 16-bit hi part and
 //     a 16-bit lo part and writes both into shared memory in the SWIZZLE_NONE K-major canonical layout,
 //     where the next layer's wgmmas read them as the A operand;
-//   * weights stream from L2 through a shared-memory ring of chunks (128 output rows x 32 K x {hi, lo})
-//     with cp.async.bulk (1-D TMA) + mbarrier complete_tx; the packed image is laid out in exactly the
-//     order the warpgroups consume it, in the same canonical layout, so a chunk is one contiguous copy;
+//   * weights stream from L2 through a shared-memory ring of chunks (128 output rows x 32 K x {hi, lo};
+//     4 stages in the split modes, 18 in bf16) with cp.async.bulk (1-D TMA) + mbarrier complete_tx, issued
+//     by one producer thread that runs ahead over all of the CTA's tiles; the consumers only wait on
+//     `full` and release stages.  The packed image is laid out in exactly the order the warpgroups consume
+//     it, in the same canonical layout, so a chunk is one contiguous copy;
 //   * fp32 parity (SNB_PREC_F16X3 / BF16X3): x*w ~= xh*wh + xl*wh + xh*wl, three wgmmas per K step
 //     with fp32 accumulation -- 22 (fp16) or 16 (bf16) significand bits per operand;
 //     SNB_PREC_BF16 is the single product;
 //   * positional encodings (63->64, 27->32 columns) are computed into shared memory in the canonical
-//     layout at the start of a tile and consumed at layers 1, 5 (skip) and the direction layer, so
-//     neither concat exists;
+//     layout and consumed at layers 1, 5 (skip) and the direction layer, so neither concat exists; the
+//     xyz encoding is written at the start of a tile, the direction encoding over it once the skip
+//     layer's (l = 4) wgmmas have retired;
+//   * biases and head weights are read from the image through L1 (__ldg), not staged in shared memory;
 //   * sigma (256->1) and rgb (128->3) heads are fp32 dot products inside the epilogue (quad shuffles
 //     combine the columns a thread's neighbours hold);
 //   * the bottleneck layer (256->256, no activation, nerf.py:140) is folded into the direction layer at
@@ -50,8 +55,11 @@ constexpr int kTile = 128;             // points per CTA tile
 constexpr int kNh = 128;               // output columns per wgmma (N); a 256-wide layer is two halves
 constexpr int kKc = 32;                // K per weight chunk
 constexpr uint32_t kStepBytes = kNh * 16 * 2;   // one K16 step of one of {hi, lo} of a chunk
-constexpr int kWgs = 2;                // warpgroups, 64 tile rows each
-constexpr int kThreads = kWgs * 128;
+constexpr int kWgs = 2;                // consumer warpgroups, 64 tile rows each
+constexpr int kThreads = (kWgs + 1) * 128;   // + one producer warpgroup
+constexpr int kProducerRegs = 24, kConsumerRegs = 240;   // setmaxnreg: 128 x 24 + 256 x 240 <= 64 K registers
+static_assert(128 * kProducerRegs + kWgs * 128 * kConsumerRegs <= 65536, "register file");
+constexpr size_t kSmemOptIn = 232448;  // opt-in dynamic shared memory per block on sm_90
 
 enum { SRC_ENC = 0, SRC_HID = 1, SRC_DIR = 2 };
 
@@ -347,19 +355,23 @@ int launch_pack_tc(const float* const* params, int precision, int new_activation
 }
 
 // ------------------------------------------------------------------ shared memory
+// The direction encoding has no buffer of its own: it is written over the first kDirPad columns of `enc` once the
+// layer-4 wgmmas (the last reader of the xyz encoding) have retired.  Biases and head weights are read from the
+// image (__ldg), not staged.  The ring takes every stage that fits in what is left.
 template <bool kSplit>
 struct TcSmem {
   static constexpr int kParts = kSplit ? 2 : 1;
   static constexpr uint32_t kStageBytes = kStepBytes * (kKc / 16) * kParts;   // one full chunk
-  // what is left of the 227 KB after the activation buffers
-  static constexpr int kStages = kSplit ? 2 : 6;
+  static constexpr size_t kActBytes = (size_t)kParts * kTile * (kWidth + kXyzPad) * 2;
+  static constexpr int kStages = (int)((kSmemOptIn - 128 - kActBytes) / (kStageBytes + 2 * sizeof(uint64_t)));
   alignas(128) unsigned char ring[kStages][kStageBytes];
   alignas(128) unsigned char hid[kParts][kTile * kWidth * 2];    // canonical [k8][row][8] hi (, lo)
-  alignas(128) unsigned char enc[kParts][kTile * kXyzPad * 2];
-  alignas(128) unsigned char dir[kParts][kTile * kDirPad * 2];
-  alignas(16) float cst[kConstFloats];
+  alignas(128) unsigned char enc[kParts][kTile * kXyzPad * 2];   // xyz encoding, then the direction encoding
   uint64_t full[kStages], empty[kStages];
 };
+static_assert(kDirPad <= kXyzPad, "the direction encoding fits in the xyz encoding's buffer");
+static_assert(sizeof(TcSmem<true>) + 128 <= kSmemOptIn && sizeof(TcSmem<false>) + 128 <= kSmemOptIn, "shared memory");
+static_assert(TcSmem<true>::kStages >= 4 && TcSmem<false>::kStages >= 6, "weight ring depth");
 
 struct TcParams {
   const unsigned char* image;
@@ -395,7 +407,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
   static_assert(!(kTrain != 0 && kEmbedded), "the training forward is the fused (rays, z) entry only");
   using Smem = TcSmem<kSplit>;
   extern __shared__ unsigned char smem_raw[];
-  Smem& s = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  Smem& s = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
   constexpr ConstLayout CL = make_const_layout();
   constexpr int kStages = Smem::kStages;
   constexpr int kParts = Smem::kParts;
@@ -408,31 +420,37 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
   const long long ntiles = (p.n_points + kTile - 1) / kTile;
   const int n_chunks = p.sigma_only ? tab.n_sigma_only : tab.n_total;
 
-  for (int i = tid; i < kConstFloats; i += kThreads) s.cst[i] = g_cst[i];
   if (tid == 0) {
     for (int i = 0; i < kStages; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], kWgs * 4); }
     fence_mbar_init();
   }
   __syncthreads();
 
-  // ---- weight stream: thread 0 keeps the ring kStages chunks ahead of consumption; a stage is refilled once
-  // all eight warps have released it
-  const long long my_tiles = ntiles > (long long)blockIdx.x ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
-  const long long n_loads = my_tiles * n_chunks;
-  long long next_load = 0;
-  auto produce = [&](long long upto) {
-    for (; next_load < n_loads && next_load < upto; ++next_load) {
-      const uint32_t st = (uint32_t)(next_load % kStages), ph = (uint32_t)(next_load / kStages) & 1;
-      mbar_wait(&s.empty[st], ph ^ 1);
-      const Chunk c = tab.c[next_load % n_chunks];
-      const uint32_t bytes = kStepBytes * kParts * c.steps;
-      mbar_arrive_expect_tx(&s.full[st], bytes);
-      bulk_g2s(s.ring[st], g_chunks + (size_t)c.off * (kStepBytes * kParts), bytes, &s.full[st]);
+  if (warp >= kWgs * 4) {
+    // ======================= producer warpgroup: one thread keeps the ring kStages chunks ahead of consumption
+    // over all of the CTA's tiles; a stage is refilled once all eight consumer warps have released it.  No
+    // consumer thread ever waits on `empty`.
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kWgs * 4 && elect_one()) {
+      const long long my_tiles = ntiles > (long long)blockIdx.x ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+      const long long n_loads = my_tiles * n_chunks;
+      uint32_t st = 0, ph = 0;
+      int ci = 0;
+      for (long long i = 0; i < n_loads; ++i) {
+        mbar_wait(&s.empty[st], ph ^ 1);
+        const Chunk c = tab.c[ci];
+        const uint32_t bytes = kStepBytes * kParts * c.steps;
+        mbar_arrive_expect_tx(&s.full[st], bytes);
+        bulk_g2s(s.ring[st], g_chunks + (size_t)c.off * (kStepBytes * kParts), bytes, &s.full[st]);
+        if (++ci == n_chunks) ci = 0;
+        if (++st == kStages) { st = 0; ph ^= 1; }
+      }
     }
-  };
-  if (tid == 0) produce(kStages);
+    return;
+  }
+  setmaxnreg_inc<kConsumerRegs>();
 
-  // ======================= warpgroups =======================
+  // ======================= consumer warpgroups =======================
   const int wgi = warp >> 2, wq = warp & 3, tq = lane & 3;
   const int r0 = wgi * 64 + wq * 16 + (lane >> 2);   // tile rows of this thread's accumulator fragments: r0, r0 + 8
   auto wg_sync = [&]() { named_bar_sync(1 + wgi, 128); };
@@ -485,8 +503,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
         }
         if (kTrain == 2) store_cell16(xyz ? p.a_enc : p.a_dir, pt, k8, xyz ? kXyzPad : kDirPad, v8);
       }
-      if (xyz) put8(s.enc[0], s.enc[kSplit ? 1 : 0], k8, r, v8);
-      else put8(s.dir[0], s.dir[kSplit ? 1 : 0], k8, r, v8);
+      put8(s.enc[0], s.enc[kSplit ? 1 : 0], k8, r, v8);
     };
     auto encode_all = [&](auto ltag) {
       constexpr int L = decltype(ltag)::value;            // 10 (xyz, 63 -> 64 channels) or 4 (dir, 27 -> 32)
@@ -543,8 +560,8 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
   uint32_t it = 0;
 
   // trunk epilogue of layer l (0..7): bias, ReLU, hi/lo split -> the next layer's A operand in shared memory
-  auto trunk_epilogue = [&](int l, long long pt0) {
-    const float* bias = s.cst + CL.b[l];
+  auto trunk_epilogue = [&](int l, long long tile, long long pt0) {
+    const float* bias = g_cst + CL.b[l];
     unsigned char* hb = kTrain == 2 ? p.a_h + (size_t)l * (size_t)p.ppad * (kWidth * 2) : nullptr;
     const bool sigma_layer = l == 7;
     if (sigma_layer) { sig[0] = 0.f; sig[1] = 0.f; }
@@ -555,7 +572,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int col = h * kNh + 8 * j + 2 * tq;
-        const float2 bb = *reinterpret_cast<const float2*>(bias + col);
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
           const int row = r0 + 8 * rr;
@@ -568,7 +585,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
           } else {
             x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f);
             if (sigma_layer) {
-              const float2 ww = *reinterpret_cast<const float2*>(s.cst + CL.sigma_w + col);
+              const float2 ww = __ldg(reinterpret_cast<const float2*>(g_cst + CL.sigma_w + col));
               sig[rr] = fmaf(x0, ww.x, sig[rr]); sig[rr] = fmaf(x1, ww.y, sig[rr]);
             }
             split_pair<kBf16, kSplit, true>(x0, x1, hi, lo);
@@ -607,11 +624,14 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
         float v = sig[rr];
         v += __shfl_xor_sync(0xffffffffu, v, 1);
         v += __shfl_xor_sync(0xffffffffu, v, 2);
-        sig[rr] = v + s.cst[CL.sigma_b];
+        sig[rr] = v + __ldg(g_cst + CL.sigma_b);
         const long long pt = pt0 + 8 * rr;
         if (p.sigma_only && tq == 0 && pt < p.n_points) p.out[pt] = sig[rr];
       }
     }
+    // this warpgroup's layer-4 wgmmas, the last readers of its rows of the xyz encoding, have retired: its
+    // threads 64..127 write the direction encoding of the same rows over it
+    if (l == 4 && !p.sigma_only && (tid & 127) >= 64) encode_row(tile, wgi * 64 + (tid & 127) - 64, false);
     fence_proxy_async_smem();     // generic-proxy smem writes -> visible to the next layer's wgmmas
     wg_sync();
   };
@@ -623,10 +643,10 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       const int col = 8 * j + 2 * tq;
-      const float2 bb = *reinterpret_cast<const float2*>(s.cst + CL.b[9] + col);
-      const float2 w0 = *reinterpret_cast<const float2*>(s.cst + CL.rgb_w + col);
-      const float2 w1 = *reinterpret_cast<const float2*>(s.cst + CL.rgb_w + kHalf + col);
-      const float2 w2 = *reinterpret_cast<const float2*>(s.cst + CL.rgb_w + 2 * kHalf + col);
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(g_cst + CL.b[9] + col));
+      const float2 w0 = __ldg(reinterpret_cast<const float2*>(g_cst + CL.rgb_w + col));
+      const float2 w1 = __ldg(reinterpret_cast<const float2*>(g_cst + CL.rgb_w + kHalf + col));
+      const float2 w2 = __ldg(reinterpret_cast<const float2*>(g_cst + CL.rgb_w + 2 * kHalf + col));
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const long long pt = pt0 + 8 * rr;
@@ -650,7 +670,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
         float v = a[rr][k];
         v += __shfl_xor_sync(0xffffffffu, v, 1);
         v += __shfl_xor_sync(0xffffffffu, v, 2);
-        v += s.cst[CL.rgb_b + k];
+        v += __ldg(g_cst + CL.rgb_b + k);
         c[k] = new_activation ? widened_sigmoid_f(v) : sigmoid_f(v);
       }
       const long long pt = pt0 + 8 * rr;
@@ -660,14 +680,10 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
 
   for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const long long pt0 = tile * kTile + r0;
-    // ---- encodings of this warpgroup's 64 rows: threads 0..63 xyz, 64..127 dir
-    {
-      const int e = tid & 127;
-      if (e < 64) encode_row(tile, wgi * 64 + e, true);
-      else if (!p.sigma_only) encode_row(tile, wgi * 64 + e - 64, false);
-      fence_proxy_async_smem();
-      wg_sync();
-    }
+    // ---- xyz encoding of this warpgroup's 64 rows (threads 0..63; the direction encoding follows layer 4)
+    if ((tid & 127) < 64) encode_row(tile, wgi * 64 + (tid & 127), true);
+    fence_proxy_async_smem();
+    wg_sync();
     int pend = -1;    // ring stage whose wgmmas are committed but not yet released
     for (int ci = 0; ci < n_chunks; ++ci, ++it) {
       const Chunk c = tab.c[ci];
@@ -681,8 +697,8 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
       mbar_wait(&s.full[st], ph);
       wgmma_fence();
       const uint32_t bh = smem_u32(s.ring[st]), bl = bh + kStepBytes * c.steps;
-      const unsigned char* abuf = c.src == SRC_HID ? s.hid[0] : (c.src == SRC_ENC ? s.enc[0] : s.dir[0]);
-      const uint32_t part = c.src == SRC_HID ? (uint32_t)sizeof(s.hid[0]) : (c.src == SRC_ENC ? (uint32_t)sizeof(s.enc[0]) : (uint32_t)sizeof(s.dir[0]));
+      const unsigned char* abuf = c.src == SRC_HID ? s.hid[0] : s.enc[0];   // SRC_ENC and SRC_DIR share `enc`
+      const uint32_t part = c.src == SRC_HID ? (uint32_t)sizeof(s.hid[0]) : (uint32_t)sizeof(s.enc[0]);
       const uint32_t ah = smem_u32(abuf) + wgi * 64 * 16 + (uint32_t)c.a16 * 2 * (kTile * 16);
 #pragma unroll
       for (int ks = 0; ks < kKc / 16; ++ks) {
@@ -697,14 +713,13 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
       wgmma_wait<1>();                                      // the previous chunk's wgmmas have retired
       if (pend >= 0 && lane == 0) mbar_arrive(&s.empty[pend]);
       pend = (int)st;
-      if (tid == 0) produce((long long)it + kStages);
       __syncwarp();
       if (ci + 1 == n_chunks || tab.c[ci + 1].layer != c.layer) {
         wgmma_wait<0>();
         if (lane == 0) mbar_arrive(&s.empty[pend]);
         pend = -1;
         if (c.layer == 9) dir_epilogue(pt0);
-        else trunk_epilogue(c.layer, pt0);
+        else trunk_epilogue(c.layer, tile, pt0);
       }
     }
   }
@@ -716,7 +731,7 @@ static int launch_tc(const TcParams& p, cudaStream_t st) {
   static SmemOptIn optin;
   const long long ntiles = (p.n_points + kTile - 1) / kTile;
   if (ntiles == 0) return SNB_OK;       // an empty pass is a no-op: no CUDA call at all
-  const size_t smem = sizeof(TcSmem<kSplit>) + 1024;
+  const size_t smem = sizeof(TcSmem<kSplit>) + 128;
   auto kern = field_tc_kernel<kBf16, kSplit, kEmbedded, kTrain>;
   if (int rc = ensure_smem(kern, optin, (int)smem, "field_tc")) return rc;
   long long ctas = sm_count();

@@ -58,6 +58,13 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+
+// per-warpgroup register budget (multiple of 8 in [24, 256]); all four warps of the warpgroup execute it
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // make generic-proxy smem writes visible to the async proxy (wgmma operand reads, TMA)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
