@@ -11,7 +11,9 @@
 //   * a layer's whole 64 x 256 fp32 accumulator lives in registers (two N = 128 halves, 128 registers
 //     per thread); the epilogue adds the bias, applies ReLU, splits the value into a 16-bit hi part and
 //     a 16-bit lo part and writes both into shared memory in the SWIZZLE_NONE K-major canonical layout,
-//     where the next layer's wgmmas read them as the A operand;
+//     where the next layer's wgmmas read them as the A operand.  The consumers' layer schedule is unrolled at
+//     compile time: chunk sources, offsets and accumulators are constants, each layer kind has its own epilogue,
+//     and the first wgmma of a (layer, half) writes its accumulator without reading it (scale-d = 0);
 //   * weights stream from L2 through a shared-memory ring of chunks (128 output rows x 32 K x {hi, lo};
 //     4 stages in the split modes, 18 in bf16) with cp.async.bulk (1-D TMA) + mbarrier complete_tx, issued
 //     by one producer thread that runs ahead over all of the CTA's tiles; the consumers only wait on
@@ -23,8 +25,8 @@
 //   * positional encodings (63->64, 27->32 columns) are computed into shared memory in the canonical
 //     layout and consumed at layers 1, 5 (skip) and the direction layer, so neither concat exists; the
 //     xyz encoding is written at the start of a tile, the direction encoding over it once the skip
-//     layer's (l = 4) wgmmas have retired;
-//   * biases and head weights are read from the image through L1 (__ldg), not staged in shared memory;
+//     layer's (l = 4) wgmmas have retired; two threads per row share a row's channels;
+//   * biases and head weights are read from the image through L1, not staged in shared memory;
 //   * sigma (256->1) and rgb (128->3) heads are fp32 dot products inside the epilogue (quad shuffles
 //     combine the columns a thread's neighbours hold);
 //   * the bottleneck layer (256->256, no activation, nerf.py:140) is folded into the direction layer at
@@ -38,6 +40,7 @@
 // Roofline: tensor pipe.  Executed MMA FLOPs are 3x the algorithmic 1 186 816 FLOP/point in the
 // split modes.  HBM traffic: 4 B/point in (z) + 16 B/point out; weights (2.2 MB per tile pass)
 // are L2 hits.
+#include <stddef.h>
 #include <stdlib.h>
 
 #include <type_traits>
@@ -120,6 +123,32 @@ __constant__ ChunkTable c_chunks = make_chunk_table();
 static constexpr ChunkTable h_chunks = make_chunk_table();
 static_assert(h_chunks.n_total == 129 && h_chunks.n_sigma_only == 120, "chunk schedule (K32)");
 static_assert(h_chunks.steps_total == 258, "K16 steps per tile");
+// first chunk and number of chunks of (layer, half) in the schedule
+__host__ __device__ constexpr int chunk_index(int l, int half) {
+  for (int i = 0; i < h_chunks.n_total; ++i)
+    if (h_chunks.c[i].layer == l && h_chunks.c[i].half == half) return i;
+  return -1;
+}
+__host__ __device__ constexpr int chunk_count(int l, int half) {
+  int n = 0;
+  for (int i = 0; i < h_chunks.n_total; ++i) n += h_chunks.c[i].layer == l && h_chunks.c[i].half == half;
+  return n;
+}
+static_assert(chunk_count(4, 0) == 10 && chunk_count(9, 0) == 9 && chunk_count(9, 1) == 0, "chunk schedule");
+// layers 1-3, 5 and 6 consume their chunks exactly like layer 1 (only the image offsets differ), so the consumers
+// run them with one copy of layer 1's code
+__host__ __device__ constexpr bool same_schedule_as_layer1(int l) {
+  for (int h = 0; h < 2; ++h) {
+    if (chunk_count(l, h) != chunk_count(1, h)) return false;
+    for (int i = 0; i < chunk_count(1, h); ++i) {
+      const Chunk a = h_chunks.c[chunk_index(1, h) + i], b = h_chunks.c[chunk_index(l, h) + i];
+      if (a.half != b.half || a.src != b.src || a.a16 != b.a16 || a.steps != b.steps || a.first != b.first) return false;
+    }
+  }
+  return true;
+}
+static_assert(same_schedule_as_layer1(2) && same_schedule_as_layer1(3) && same_schedule_as_layer1(5) &&
+              same_schedule_as_layer1(6), "plain layers share layer 1's schedule");
 
 // ------------------------------------------------------------------ packed image
 // [PackedHeader 256 B][consts: biases + head weights, fp32][chunk 0][chunk 1]...
@@ -139,6 +168,12 @@ __host__ __device__ constexpr ConstLayout make_const_layout() {
   return L;
 }
 constexpr int kConstFloats = make_const_layout().total;
+__host__ __device__ constexpr bool trunk_biases_strided() {   // the trunk epilogue computes CL.b[l] as l * kWidth
+  for (int l = 0; l < 8; ++l)
+    if (make_const_layout().b[l] != l * kWidth) return false;
+  return true;
+}
+static_assert(trunk_biases_strided(), "trunk layer l's bias starts at l * kWidth in the image's constants");
 constexpr size_t kConstBytes = (size_t)kConstFloats * 4;
 
 __host__ __device__ constexpr bool prec_split(int precision) { return precision != SNB_PREC_BF16; }
@@ -155,12 +190,25 @@ size_t tc_packed_bytes(int precision) {
   return sizeof(PackedHeader) + kConstBytes + chunks_bytes(precision) + kFusedFloats * sizeof(float);
 }
 
+// lambdas of the unrolled consumer schedule must inline: an accumulator array passed to an out-of-line call would
+// live in local memory
+#define SNB_INLINE __attribute__((always_inline))
+
 template <class F, int... I>
 __device__ __forceinline__ void static_for_impl(F&& f, std::integer_sequence<int, I...>) {
   (f(std::integral_constant<int, I>{}), ...);
 }
 template <int N, class F>
 __device__ __forceinline__ void static_for(F&& f) { static_for_impl(f, std::make_integer_sequence<int, N>{}); }
+
+// A read-only float2 from global memory as a volatile load, so the front end does not hoist an epilogue's bias loads
+// into the preceding MMA issue, where their registers push other values out to local memory.  (ptxas still moves
+// some of them up; DESIGN.md §4.1 lists the spills that remain.)
+__device__ __forceinline__ float2 ldg_f2_here(const float* p) {
+  float2 v;
+  asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
+  return v;
+}
 
 // 16-bit conversions -------------------------------------------------------------------
 template <bool kBf16>
@@ -451,12 +499,22 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
   setmaxnreg_inc<kConsumerRegs>();
 
   // ======================= consumer warpgroups =======================
+  // The layer schedule is unrolled at compile time: every chunk's A source, K offset, step count and accumulator
+  // register set are constants, and a layer's first wgmma (scale-d = 0) is the only write of its accumulator.
   const int wgi = warp >> 2, wq = warp & 3, tq = lane & 3;
   const int r0 = wgi * 64 + wq * 16 + (lane >> 2);   // tile rows of this thread's accumulator fragments: r0, r0 + 8
   auto wg_sync = [&]() { named_bar_sync(1 + wgi, 128); };
+  constexpr uint32_t kHidPart = kTile * kWidth * 2, kEncPart = kTile * kXyzPad * 2;   // bytes of one of {hi, lo}
+  // shared-window addresses are one base plus compile-time offsets, so they cost few registers
+  constexpr uint32_t kOffRing = offsetof(Smem, ring), kOffHid = offsetof(Smem, hid), kOffEnc = offsetof(Smem, enc);
+  const uint32_t sbase = smem_u32(&s);
+  const uint32_t a_wg = sbase + wgi * 64 * 16;              // this warpgroup's A rows (+ kOffHid / kOffEnc)
+  const uint32_t hid_thr = sbase + kOffHid + r0 * 16 + tq * 4;   // canon_off(r0, 2 tq): this thread's first epilogue word
+  // encodings: the tile row and the half of its channels this thread computes (all 128 threads of a warpgroup)
+  const int er = wgi * 64 + (tid & 63), epart = (tid >> 6) & 1;
 
   // 16-bit storage: 8 consecutive features of one point -> one 16-byte cell of a T32 tensor
-  auto store_cell16 = [&](unsigned char* base, long long pt, int f8, int F, const float (&v)[8]) {
+  auto store_cell16 = [&](unsigned char* base, long long pt, int f8, int F, const float (&v)[8]) SNB_INLINE {
     if (pt >= p.ppad) return;
     const bool live = pt < p.n_points;
     uint4 c;
@@ -464,128 +522,181 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
     c.z = live ? pack_half2_sat(v[4], v[5]) : 0u; c.w = live ? pack_half2_sat(v[6], v[7]) : 0u;
     *reinterpret_cast<uint4*>(base + a16_cell(pt, f8, F)) = c;
   };
-  // 8 consecutive channels (one 16-byte core-matrix row of tile row `r`) -> hi (and lo) vector stores, canonical layout
-  auto put8 = [&](unsigned char* hi_base, unsigned char* lo_base, int k8, int r, const float (&v)[8]) {
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) split_pair<kBf16, kSplit>(v[2 * j], v[2 * j + 1], h[j], l[j]);
-    const uint32_t off = (uint32_t)k8 * (kTile * 16) + r * 16;
-    *reinterpret_cast<uint4*>(hi_base + off) = make_uint4(h[0], h[1], h[2], h[3]);
-    if (kSplit) *reinterpret_cast<uint4*>(lo_base + off) = make_uint4(l[0], l[1], l[2], l[3]);
-  };
-  // positional encoding of tile row r: xyz (Embedding(3, 10) of o + d z) or dir (Embedding(3, 4) of d)
-  auto encode_row = [&](long long tile, int r, bool xyz) {
-    const long long pt = tile * kTile + r;
-    const bool live = pt < p.n_points;
-    float x[3] = {0.f, 0.f, 0.f};
-    const float* xr = nullptr;
-    if (kEmbedded) {
-      xr = p.x + pt * p.x_stride;
-    } else if (live) {
+
+  // the encoder thread's ray (o, d) and sample depth, loaded one tile ahead (before the direction layer of the
+  // previous tile) so the HBM latency hides under that layer's MMAs
+  struct RowIn { float4 q0, q1; float z; };
+  RowIn in{};
+  auto load_row = [&](long long tile) SNB_INLINE {
+    const long long pt = tile * kTile + er;
+    if (!kEmbedded && tile < ntiles && pt < p.n_points) {
       const long long ray = pt / p.n_samples;
-      const float4 q0 = *reinterpret_cast<const float4*>(p.rays + ray * 8);
-      const float4 q1 = *reinterpret_cast<const float4*>(p.rays + ray * 8 + 4);
-      if (xyz) {
-        const float zz = p.z[pt];
-        x[0] = __fadd_rn(q0.x, __fmul_rn(q0.w, zz));   // rendering.py:284-285 rounding
-        x[1] = __fadd_rn(q0.y, __fmul_rn(q1.x, zz));
-        x[2] = __fadd_rn(q0.z, __fmul_rn(q1.y, zz));
-      } else {
-        x[0] = q0.w; x[1] = q1.x; x[2] = q1.y;          // ray direction (not normalised, rendering.py:261)
-      }
+      in.q0 = *reinterpret_cast<const float4*>(p.rays + ray * 8);
+      in.q1 = *reinterpret_cast<const float4*>(p.rays + ray * 8 + 4);
+      in.z = p.z[pt];
     }
-    auto emit = [&](auto ktag, const float (&v8)[8]) {
-      constexpr int k8 = decltype(ktag)::value;
+  };
+  // positional encoding of tile row er, channels [32 P, 32 P + 32) of the xyz encoding (Embedding(3, 10) of
+  // o + d z) or [16 P, 16 P + 16) of the direction encoding (Embedding(3, 4) of d)
+  auto encode = [&](auto ltag, auto ptag, long long tile) SNB_INLINE {
+    constexpr int L = decltype(ltag)::value, P = decltype(ptag)::value;
+    constexpr bool kXyz = L == SNB_XYZ_FREQS;
+    constexpr int kCh = 3 * (2 * L + 1), kPad = (kCh + 7) / 8 * 8, kK8 = kPad / 16;   // k8 groups per thread
+    constexpr int c_lo = 8 * kK8 * P, c_hi = 8 * kK8 * (P + 1);
+    const long long pt = tile * kTile + er;
+    const bool live = pt < p.n_points;
+    float v[kPad];
+#pragma unroll
+    for (int j = 0; j < kPad; ++j) v[j] = 0.f;
+    if (kEmbedded) {
+      const float* xr = p.x + pt * p.x_stride;
+      const int nin = p.sigma_only ? kXyzCh : kXyzCh + kDirCh;
+#pragma unroll
+      for (int j = c_lo; j < (c_hi < kCh ? c_hi : kCh); ++j) {
+        const int col = kXyz ? j : kXyzCh + j;
+        v[j] = (live && col < nin) ? xr[col] : 0.f;
+      }
+    } else {
+      float x[3] = {0.f, 0.f, 0.f};
+      if (live) {
+        if (kXyz) {
+          x[0] = __fadd_rn(in.q0.x, __fmul_rn(in.q0.w, in.z));   // rendering.py:284-285 rounding
+          x[1] = __fadd_rn(in.q0.y, __fmul_rn(in.q1.x, in.z));
+          x[2] = __fadd_rn(in.q0.z, __fmul_rn(in.q1.y, in.z));
+        } else {
+          x[0] = in.q0.w; x[1] = in.q1.x; x[2] = in.q1.y;      // ray direction (not normalised, rendering.py:261)
+        }
+      }
+      v[0] = x[0]; v[1] = x[1]; v[2] = x[2];
+#pragma unroll
+      for (int f = 0; f < L; ++f)
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const int cs = 3 + 6 * f + c, cc = cs + 3;     // channels of sin and cos
+          if ((cs >= c_lo && cs < c_hi) || (cc >= c_lo && cc < c_hi)) {
+            float sn, cs_;
+            if (kSplit) sincosf(x[c] * (float)(1 << f), &sn, &cs_);
+            else sincos_fast(x[c] * (float)(1 << f), &sn, &cs_);
+            v[cs] = sn;
+            v[cc] = cs_;
+          }
+        }
+    }
+    static_for<kK8>([&](auto ktag) SNB_INLINE {
+      constexpr int k8 = kK8 * P + decltype(ktag)::value;
+      const float v8[8] = {v[8 * k8], v[8 * k8 + 1], v[8 * k8 + 2], v[8 * k8 + 3], v[8 * k8 + 4], v[8 * k8 + 5], v[8 * k8 + 6], v[8 * k8 + 7]};
       if (!kEmbedded) {
         if (kTrain == 1 && live) {
-          float4* dst = reinterpret_cast<float4*>((xyz ? p.save_enc + pt * kXyzPad : p.save_dir + pt * kDirPad) + k8 * 8);
+          float4* dst = reinterpret_cast<float4*>((kXyz ? p.save_enc + pt * kXyzPad : p.save_dir + pt * kDirPad) + k8 * 8);
           dst[0] = make_float4(v8[0], v8[1], v8[2], v8[3]); dst[1] = make_float4(v8[4], v8[5], v8[6], v8[7]);
         }
-        if (kTrain == 2) store_cell16(xyz ? p.a_enc : p.a_dir, pt, k8, xyz ? kXyzPad : kDirPad, v8);
+        if (kTrain == 2) store_cell16(kXyz ? p.a_enc : p.a_dir, pt, k8, kXyz ? kXyzPad : kDirPad, v8);
       }
-      put8(s.enc[0], s.enc[kSplit ? 1 : 0], k8, r, v8);
-    };
-    auto encode_all = [&](auto ltag) {
-      constexpr int L = decltype(ltag)::value;            // 10 (xyz, 63 -> 64 channels) or 4 (dir, 27 -> 32)
-      constexpr int kCh = 3 * (2 * L + 1), kPad = (kCh + 7) / 8 * 8;
-      float v[kPad];
+      uint32_t h[4], l[4];
 #pragma unroll
-      for (int j = 0; j < kPad; ++j) v[j] = 0.f;
-      if (kEmbedded) {
-        const int nin = p.sigma_only ? kXyzCh : kXyzCh + kDirCh;
-#pragma unroll
-        for (int j = 0; j < kCh; ++j) {
-          const int col = L == SNB_XYZ_FREQS ? j : kXyzCh + j;
-          v[j] = (live && col < nin) ? xr[col] : 0.f;
-        }
-      } else {
-        v[0] = x[0]; v[1] = x[1]; v[2] = x[2];
-#pragma unroll
-        for (int f = 0; f < L; ++f)
-#pragma unroll
-          for (int c = 0; c < 3; ++c) {
-            float sn, cs;
-            if (kSplit) sincosf(x[c] * (float)(1 << f), &sn, &cs);
-            else sincos_fast(x[c] * (float)(1 << f), &sn, &cs);
-            v[3 + 6 * f + c] = sn;
-            v[3 + 6 * f + 3 + c] = cs;
-          }
-      }
-      static_for<kPad / 8>([&](auto ktag) {
-        constexpr int k8 = decltype(ktag)::value;
-        const float v8[8] = {v[8 * k8], v[8 * k8 + 1], v[8 * k8 + 2], v[8 * k8 + 3], v[8 * k8 + 4], v[8 * k8 + 5], v[8 * k8 + 6], v[8 * k8 + 7]};
-        emit(ktag, v8);
-      });
-    };
-    if (xyz) encode_all(std::integral_constant<int, SNB_XYZ_FREQS>{});
-    else encode_all(std::integral_constant<int, SNB_DIR_FREQS>{});
+      for (int j = 0; j < 4; ++j) split_pair<kBf16, kSplit>(v8[2 * j], v8[2 * j + 1], h[j], l[j]);
+      const uint32_t a = sbase + kOffEnc + k8 * (kTile * 16) + er * 16;
+      st_shared_v4(a, h[0], h[1], h[2], h[3]);
+      if (kSplit) st_shared_v4(a + kEncPart, l[0], l[1], l[2], l[3]);
+    });
+  };
+  auto encode_rows = [&](auto ltag, long long tile) SNB_INLINE {
+    if (epart == 0) encode(ltag, std::integral_constant<int, 0>{}, tile);
+    else encode(ltag, std::integral_constant<int, 1>{}, tile);
   };
 
-  auto mma = [&](float (&d)[64], uint64_t a, uint64_t b, uint32_t accumulate) {
-    if (kBf16) wgmma_m64n128_bf16(d, a, b, accumulate);
-    else wgmma_m64n128_f16(d, a, b, accumulate);
+  auto mma = [&](float (&d)[64], uint64_t a, uint64_t b, bool first) SNB_INLINE {
+    if (first) {                 // accumulate = 0, D write-only
+      if (kBf16) wgmma_m64n128_bf16_first(d, a, b);
+      else wgmma_m64n128_f16_first(d, a, b);
+    } else {
+      if (kBf16) wgmma_m64n128_bf16(d, a, b, 1u);
+      else wgmma_m64n128_f16(d, a, b, 1u);
+    }
   };
-  // K16 step ks of the current chunk into accumulator d: hi*hi (+ lo*hi + hi*lo)
-  auto issue_step = [&](float (&d)[64], uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl, uint32_t accumulate) {
+  // K16 step of a chunk into accumulator d: hi*hi (+ lo*hi + hi*lo); `first` starts the (layer, half)
+  auto issue_step = [&](float (&d)[64], uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl, bool first) SNB_INLINE {
     const uint64_t da_h = make_smem_desc(ah, kTile * 16, 128), db_h = make_smem_desc(bh, kNh * 16, 128);
-    mma(d, da_h, db_h, accumulate);
+    mma(d, da_h, db_h, first);
     if (kSplit) {
-      mma(d, make_smem_desc(al, kTile * 16, 128), db_h, 1u);
-      mma(d, da_h, make_smem_desc(bl, kNh * 16, 128), 1u);
+      mma(d, make_smem_desc(al, kTile * 16, 128), db_h, false);
+      mma(d, da_h, make_smem_desc(bl, kNh * 16, 128), false);
     }
   };
 
-  float acc0[64], acc1[64];
-  float sig[2] = {0.f, 0.f};     // sigma of rows r0, r0 + 8 (layer 8's epilogue -> the direction layer's)
-  uint32_t it = 0;
+  // Ring position of the next chunk.  Chunks are consumed in exactly the producer's order; the stage of chunk i is
+  // released once the wgmmas of chunk i + 1 are committed and chunk i's have retired (or at the layer's drain).
+  uint32_t st = 0, ph = 0;
+  auto prev_stage = [&]() { return st == 0 ? (uint32_t)kStages - 1 : st - 1; };
+  auto issue_chunk = [&](auto ctag, float (&d)[64]) SNB_INLINE {
+    constexpr Chunk c = h_chunks.c[decltype(ctag)::value];
+    mbar_wait(&s.full[st], ph);
+    wgmma_fence();
+    const uint32_t bh = sbase + kOffRing + st * Smem::kStageBytes, bl = bh + kStepBytes * c.steps;
+    // the A base goes through an opaque move: otherwise the compiler computes the descriptors of every chunk once,
+    // shares them between layers (they repeat) and keeps them live across the tile, out of the accumulators' registers
+    uint32_t abase;
+    asm volatile("mov.b32 %0, %1;" : "=r"(abase) : "r"(a_wg));
+    const uint32_t ah = abase + (c.src == SRC_HID ? kOffHid : kOffEnc) + c.a16 * 2 * (kTile * 16);
+    constexpr uint32_t part = c.src == SRC_HID ? kHidPart : kEncPart;
+    static_for<c.steps>([&](auto ktag) SNB_INLINE {
+      constexpr int ks = decltype(ktag)::value;
+      issue_step(d, ah + ks * 2 * (kTile * 16), ah + ks * 2 * (kTile * 16) + part, bh + ks * kStepBytes,
+                 bl + ks * kStepBytes, ks == 0 && c.first);
+    });
+    wgmma_commit();
+    if (!(c.first && c.half == 0)) {       // a layer's first chunk follows a drain: nothing to release
+      wgmma_wait<1>();                      // the previous chunk's wgmmas have retired
+      if (lane == 0) mbar_arrive(&s.empty[prev_stage()]);
+      __syncwarp();
+    }
+    if (++st == kStages) { st = 0; ph ^= 1; }
+  };
+  auto issue_range = [&](auto c0tag, auto ntag, float (&d)[64]) SNB_INLINE {
+    static_for<decltype(ntag)::value>([&](auto i) SNB_INLINE {
+      issue_chunk(std::integral_constant<int, decltype(c0tag)::value + decltype(i)::value>{}, d);
+    });
+  };
+  auto drain = [&]() {                      // all of a layer's wgmmas have retired
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(&s.empty[prev_stage()]);
+    __syncwarp();
+  };
 
-  // trunk epilogue of layer l (0..7): bias, ReLU, hi/lo split -> the next layer's A operand in shared memory
-  auto trunk_epilogue = [&](int l, long long tile, long long pt0) {
-    const float* bias = g_cst + CL.b[l];
-    unsigned char* hb = kTrain == 2 ? p.a_h + (size_t)l * (size_t)p.ppad * (kWidth * 2) : nullptr;
-    const bool sigma_layer = l == 7;
-    if (sigma_layer) { sig[0] = 0.f; sig[1] = 0.f; }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float (&d)[64] = h ? acc1 : acc0;
+  float acc[2][64];              // a layer's two N = 128 halves
+  float sig[2] = {0.f, 0.f};     // sigma of rows r0, r0 + 8 (layer 7's epilogue -> the direction layer's)
+
+  // trunk epilogue of layer l (0..7): bias, ReLU, hi/lo split -> the next layer's A operand in shared memory.
+  // L is the layer kind: 4 (skip layer: then writes the direction encoding), 7 (sigma head) or any other layer.
+  auto trunk_epilogue = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
+    constexpr int L = decltype(ltag)::value;
+    constexpr bool kSigma = L == 7;
+    const float* bias = g_cst + l * kWidth;            // CL.b[l]
+    // kTrain == 2: the fp16 activation words and ReLU mask words are kept in registers and stored to global memory
+    // after the barrier that ends the epilogue; stored inside it, they made the epilogue's `fence.proxy.async`
+    // (MEMBAR.ALL.CTA) wait for their completion in every layer
+    uint32_t h16v[2][16][2], mwv[2][4][2];
+    if (kSigma) { sig[0] = 0.f; sig[1] = 0.f; }
+    static_for<2>([&](auto htag) SNB_INLINE {
+      constexpr int h = decltype(htag)::value;
+      float (&d)[64] = acc[h];
       uint32_t mw[2] = {0u, 0u};
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
+      static_for<16>([&](auto jtag) SNB_INLINE {
+        constexpr int j = decltype(jtag)::value;
         const int col = h * kNh + 8 * j + 2 * tq;
-        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
+        const float2 bb = ldg_f2_here(bias + col);
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
-          const int row = r0 + 8 * rr;
           const long long pt = pt0 + 8 * rr;
           float x0 = d[4 * j + 2 * rr] + bb.x, x1 = d[4 * j + 2 * rr + 1] + bb.y;
           uint32_t hi, lo;
-          if (kTrain == 0 && !sigma_layer) {
+          if (kTrain == 0 && !kSigma) {
             // nobody needs the fp32 post-activation value: ReLU and the fp16 range guard ride on the converts
             split_pair_relu<kBf16, kSplit>(x0, x1, hi, lo);
           } else {
             x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f);
-            if (sigma_layer) {
-              const float2 ww = __ldg(reinterpret_cast<const float2*>(g_cst + CL.sigma_w + col));
+            if (kSigma) {
+              const float2 ww = ldg_f2_here(g_cst + CL.sigma_w + col);
               sig[rr] = fmaf(x0, ww.x, sig[rr]); sig[rr] = fmaf(x1, ww.y, sig[rr]);
             }
             split_pair<kBf16, kSplit, true>(x0, x1, hi, lo);
@@ -593,15 +704,13 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
               *reinterpret_cast<float2*>(p.save_h + ((size_t)l * p.n_points + pt) * kWidth + col) = make_float2(x0, x1);
             if (kTrain == 2) {
               // fp16 modes: the hi word of the split IS rn_fp16(value) (saturated); bf16 modes convert separately
-              const uint32_t h16 = kBf16 ? pack_half2_sat(x0, x1) : hi;
-              if (pt < p.ppad)
-                *reinterpret_cast<uint32_t*>(hb + a16_cell(pt, col >> 3, kWidth) + (col & 7) * 2) = pt < p.n_points ? h16 : 0u;
+              h16v[h][j][rr] = kBf16 ? pack_half2_sat(x0, x1) : hi;
               mw[rr] |= ((x0 > 0.f ? 1u : 0u) << (col & 31)) | ((x1 > 0.f ? 1u : 0u) << ((col & 31) + 1));
             }
           }
-          const uint32_t off = canon_off(row, col);
-          *reinterpret_cast<uint32_t*>(s.hid[0] + off) = hi;
-          if (kSplit) *reinterpret_cast<uint32_t*>(s.hid[kSplit ? 1 : 0] + off) = lo;
+          const uint32_t a = hid_thr + (h * 16 + j) * (kTile * 16) + rr * 128;   // canon_off(r0 + 8 rr, col)
+          st_shared_u32(a, hi);
+          if (kSplit) st_shared_u32(a + kHidPart, lo);
         }
         if (kTrain == 2 && (j & 3) == 3) {
           // a 32-column group is complete: the quad's four threads hold its 32 ReLU bits of each row
@@ -610,14 +719,13 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
             uint32_t w = mw[rr];
             w |= __shfl_xor_sync(0xffffffffu, w, 1);
             w |= __shfl_xor_sync(0xffffffffu, w, 2);
-            const long long pt = pt0 + 8 * rr;
-            if (tq == 0 && pt < p.ppad) p.a_mask[a16_mask_index(l, col >> 5, pt, p.ppad)] = pt < p.n_points ? w : 0u;
+            mwv[h][j / 4][rr] = w;
             mw[rr] = 0u;
           }
         }
-      }
-    }
-    if (sigma_layer) {
+      });
+    });
+    if (kSigma) {
       // sigma head (nerf.py:136): the quad's four threads hold the row's columns
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
@@ -629,15 +737,35 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
         if (p.sigma_only && tq == 0 && pt < p.n_points) p.out[pt] = sig[rr];
       }
     }
-    // this warpgroup's layer-4 wgmmas, the last readers of its rows of the xyz encoding, have retired: its
-    // threads 64..127 write the direction encoding of the same rows over it
-    if (l == 4 && !p.sigma_only && (tid & 127) >= 64) encode_row(tile, wgi * 64 + (tid & 127) - 64, false);
+    // this warpgroup's layer-4 wgmmas, the last readers of its rows of the xyz encoding, have retired: it writes
+    // the direction encoding of the same rows over it
+    if (L == 4 && !p.sigma_only) encode_rows(std::integral_constant<int, SNB_DIR_FREQS>{}, tile);
     fence_proxy_async_smem();     // generic-proxy smem writes -> visible to the next layer's wgmmas
     wg_sync();
+    if (kTrain == 2) {
+      unsigned char* hb = p.a_h + (size_t)l * (size_t)p.ppad * (kWidth * 2);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const long long pt = pt0 + 8 * rr;
+        if (pt >= p.ppad) continue;
+        const bool live = pt < p.n_points;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int col = h * kNh + 8 * j + 2 * tq;
+            *reinterpret_cast<uint32_t*>(hb + a16_cell(pt, col >> 3, kWidth) + (col & 7) * 2) = live ? h16v[h][j][rr] : 0u;
+          }
+#pragma unroll
+          for (int g = 0; g < 4; ++g)
+            if (tq == 0) p.a_mask[a16_mask_index(l, h * 4 + g, pt, p.ppad)] = live ? mwv[h][g][rr] : 0u;
+        }
+      }
+    }
   };
 
   // direction layer: shifted softplus / ReLU, rgb head (nerf.py:142-146), the [r, g, b, sigma] rows
-  auto dir_epilogue = [&](long long pt0) {
+  auto dir_epilogue = [&](const float (&d)[64], long long pt0) SNB_INLINE {
     const float sh = new_activation ? 1.0f : 0.0f;   // shifted softplus: fold the -1 into the bias
     float a[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
 #pragma unroll
@@ -650,7 +778,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const long long pt = pt0 + 8 * rr;
-        float x0 = acc0[4 * j + 2 * rr] + (bb.x - sh), x1 = acc0[4 * j + 2 * rr + 1] + (bb.y - sh);
+        float x0 = d[4 * j + 2 * rr] + (bb.x - sh), x1 = d[4 * j + 2 * rr + 1] + (bb.y - sh);
         if (new_activation) { x0 = softplus_fast(x0); x1 = softplus_fast(x1); }
         else { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
         if (kTrain == 1 && pt < p.n_points) *reinterpret_cast<float2*>(p.save_g + pt * kHalf + col) = make_float2(x0, x1);
@@ -678,50 +806,36 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
     }
   };
 
+  // one layer: its wgmmas in the schedule of layer L (layers 1-3, 5 and 6 share layer 1's), the drain, the epilogue.
+  // Each (layer, half) starts with a write-only wgmma (accumulate = 0), so no instruction writes an accumulator
+  // between a layer's first wgmma and its drain.
+  auto run_layer = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
+    constexpr int L = decltype(ltag)::value;
+    issue_range(std::integral_constant<int, chunk_index(L, 0)>{}, std::integral_constant<int, chunk_count(L, 0)>{}, acc[0]);
+    if constexpr (L != 9)
+      issue_range(std::integral_constant<int, chunk_index(L, 1)>{}, std::integral_constant<int, chunk_count(L, 1)>{}, acc[1]);
+    drain();
+    if constexpr (L == 9) dir_epilogue(acc[0], pt0);
+    else trunk_epilogue(ltag, l, tile, pt0);
+  };
+  load_row(blockIdx.x);
   for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const long long pt0 = tile * kTile + r0;
-    // ---- xyz encoding of this warpgroup's 64 rows (threads 0..63; the direction encoding follows layer 4)
-    if ((tid & 127) < 64) encode_row(tile, wgi * 64 + (tid & 127), true);
+    // ---- xyz encoding of this warpgroup's 64 rows (the direction encoding follows layer 4)
+    encode_rows(std::integral_constant<int, SNB_XYZ_FREQS>{}, tile);
     fence_proxy_async_smem();
     wg_sync();
-    int pend = -1;    // ring stage whose wgmmas are committed but not yet released
-    for (int ci = 0; ci < n_chunks; ++ci, ++it) {
-      const Chunk c = tab.c[ci];
-      if (c.first && c.half == 0) {
-        // a new layer: the accumulators are overwritten (accumulate = 0); defining them here ends their
-        // live range at the previous epilogue
-#pragma unroll
-        for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
-      }
-      const uint32_t st = it % kStages, ph = (it / kStages) & 1;
-      mbar_wait(&s.full[st], ph);
-      wgmma_fence();
-      const uint32_t bh = smem_u32(s.ring[st]), bl = bh + kStepBytes * c.steps;
-      const unsigned char* abuf = c.src == SRC_HID ? s.hid[0] : s.enc[0];   // SRC_ENC and SRC_DIR share `enc`
-      const uint32_t part = c.src == SRC_HID ? (uint32_t)sizeof(s.hid[0]) : (uint32_t)sizeof(s.enc[0]);
-      const uint32_t ah = smem_u32(abuf) + wgi * 64 * 16 + (uint32_t)c.a16 * 2 * (kTile * 16);
-#pragma unroll
-      for (int ks = 0; ks < kKc / 16; ++ks) {
-        if (ks < c.steps) {
-          const uint32_t accumulate = (ks == 0 && c.first) ? 0u : 1u;
-          const uint32_t a_k = ah + ks * 2 * (kTile * 16), b_k = ks * kStepBytes;
-          if (c.half == 0) issue_step(acc0, a_k, a_k + part, bh + b_k, bl + b_k, accumulate);
-          else issue_step(acc1, a_k, a_k + part, bh + b_k, bl + b_k, accumulate);
-        }
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                                      // the previous chunk's wgmmas have retired
-      if (pend >= 0 && lane == 0) mbar_arrive(&s.empty[pend]);
-      pend = (int)st;
-      __syncwarp();
-      if (ci + 1 == n_chunks || tab.c[ci + 1].layer != c.layer) {
-        wgmma_wait<0>();
-        if (lane == 0) mbar_arrive(&s.empty[pend]);
-        pend = -1;
-        if (c.layer == 9) dir_epilogue(pt0);
-        else trunk_epilogue(c.layer, tile, pt0);
-      }
-    }
+    // layers 0..7, then the direction layer 9 (the bottleneck, 8, is folded into it); the plain hidden layers run
+    // as loops over one copy of the code, which keeps the kernel's instruction footprint down
+    run_layer(std::integral_constant<int, 0>{}, 0, tile, pt0);
+#pragma unroll 1
+    for (int l = 1; l < 4; ++l) run_layer(std::integral_constant<int, 1>{}, l, tile, pt0);
+    run_layer(std::integral_constant<int, 4>{}, 4, tile, pt0);
+#pragma unroll 1
+    for (int l = 5; l < 7; ++l) run_layer(std::integral_constant<int, 1>{}, l, tile, pt0);
+    run_layer(std::integral_constant<int, 7>{}, 7, tile, pt0);
+    load_row(tile + gridDim.x);   // the next tile's rays and depths, under this tile's last MMAs
+    if (!p.sigma_only) run_layer(std::integral_constant<int, 9>{}, 9, tile, pt0);   // sigma-only passes end with layer 7
   }
 }
 
