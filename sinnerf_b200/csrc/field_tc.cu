@@ -12,8 +12,9 @@
 //     per thread); the epilogue adds the bias, applies ReLU, splits the value into a 16-bit hi part and
 //     a 16-bit lo part and writes both into shared memory in the SWIZZLE_NONE K-major canonical layout,
 //     where the next layer's wgmmas read them as the A operand.  The consumers' layer schedule is unrolled at
-//     compile time: chunk sources, offsets and accumulators are constants, each layer kind has its own epilogue,
-//     and the first wgmma of a (layer, half) writes its accumulator without reading it (scale-d = 0);
+//     compile time: chunk sources, offsets and accumulators are constants, and the first wgmma of a (layer, half)
+//     writes its accumulator without reading it (scale-d = 0).  The epilogue runs in 32-column blocks, each one
+//     K chunk of the next layer's input, interleaved with the wgmmas still in flight (see layer_body);
 //   * weights stream from L2 through a shared-memory ring of chunks (128 output rows x 32 K x {hi, lo};
 //     4 stages in the split modes, 18 in bf16) with cp.async.bulk (1-D TMA) + mbarrier complete_tx, issued
 //     by one producer thread that runs ahead over all of the CTA's tiles; the consumers only wait on
@@ -25,7 +26,7 @@
 //   * positional encodings (63->64, 27->32 columns) are computed into shared memory in the canonical
 //     layout and consumed at layers 1, 5 (skip) and the direction layer, so neither concat exists; the
 //     xyz encoding is written at the start of a tile, the direction encoding over it once the skip
-//     layer's (l = 4) wgmmas have retired; two threads per row share a row's channels;
+//     layer's (l = 4) enc chunks have retired; two threads per row share a row's channels;
 //   * biases and head weights are read from the image through L1, not staged in shared memory;
 //   * sigma (256->1) and rgb (128->3) heads are fp32 dot products inside the epilogue (quad shuffles
 //     combine the columns a thread's neighbours hold);
@@ -149,6 +150,28 @@ __host__ __device__ constexpr bool same_schedule_as_layer1(int l) {
 }
 static_assert(same_schedule_as_layer1(2) && same_schedule_as_layer1(3) && same_schedule_as_layer1(5) &&
               same_schedule_as_layer1(6), "plain layers share layer 1's schedule");
+// chunks of (l, 1) that read the xyz encoding; they come first
+__host__ __device__ constexpr int enc_chunks(int l) {
+  int n = 0;
+  for (int i = 0; i < chunk_count(l, 1); ++i) n += h_chunks.c[chunk_index(l, 1) + i].src == SRC_ENC;
+  return n;
+}
+// the consumers run each trunk layer's epilogue in four 32-column blocks under the wgmmas (field_tc_kernel): a
+// layer's half-0 chunks 0-3 read only enc or hid blocks 0-3, and chunk e + b of its half 1 reads hid block b
+__host__ __device__ constexpr bool epilogue_blocks_fit(int l, bool check_half1) {
+  for (int b = 0; b < 4; ++b) {
+    const Chunk a = h_chunks.c[chunk_index(l, 0) + b];
+    if (a.src == SRC_DIR || (a.src == SRC_HID && a.a16 >= 8)) return false;
+    if (!check_half1) continue;
+    const Chunk c = h_chunks.c[chunk_index(l, 1) + enc_chunks(l) + b];
+    if (c.src != SRC_HID || c.a16 != 2 * b) return false;
+  }
+  return true;
+}
+static_assert(kKc == 32 && epilogue_blocks_fit(1, true) && epilogue_blocks_fit(4, true) && epilogue_blocks_fit(7, true) &&
+              epilogue_blocks_fit(9, false) && chunk_count(1, 0) >= 4 && chunk_count(1, 1) == enc_chunks(1) + 8 &&
+              chunk_count(4, 1) == enc_chunks(4) + 8 && chunk_count(0, 1) == enc_chunks(0),
+              "epilogue blocks of 32 columns interleave with the next layer's chunks");
 
 // ------------------------------------------------------------------ packed image
 // [PackedHeader 256 B][consts: biases + head weights, fp32][chunk 0][chunk 1]...
@@ -200,6 +223,8 @@ __device__ __forceinline__ void static_for_impl(F&& f, std::integer_sequence<int
 }
 template <int N, class F>
 __device__ __forceinline__ void static_for(F&& f) { static_for_impl(f, std::make_integer_sequence<int, N>{}); }
+template <int N>
+using Int = std::integral_constant<int, N>;
 
 // A read-only float2 from global memory as a volatile load, so the front end does not hoist an epilogue's bias loads
 // into the preceding MMA issue, where their registers push other values out to local memory.  (ptxas still moves
@@ -624,12 +649,19 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
     }
   };
 
+  constexpr bool kDrained = kTrain != 0;   // the training forward keeps the drained schedule (drained_layer)
+  float acc[2][64];              // a layer's two N = 128 halves
+  float sig[2] = {0.f, 0.f};     // sigma of rows r0, r0 + 8 (layer 7's epilogue -> the direction layer's)
+
   // Ring position of the next chunk.  Chunks are consumed in exactly the producer's order; the stage of chunk i is
-  // released once the wgmmas of chunk i + 1 are committed and chunk i's have retired (or at the layer's drain).
+  // released once the wgmmas of chunk i + 1 are committed and chunk i's have retired (or at the tile's drain).
   uint32_t st = 0, ph = 0;
   auto prev_stage = [&]() { return st == 0 ? (uint32_t)kStages - 1 : st - 1; };
-  auto issue_chunk = [&](auto ctag, float (&d)[64]) SNB_INLINE {
-    constexpr Chunk c = h_chunks.c[decltype(ctag)::value];
+  // chunk ci of the schedule into the accumulator of its half; on return only its own wgmmas may still be in flight
+  auto issue = [&](auto ctag) SNB_INLINE {
+    constexpr int ci = decltype(ctag)::value;
+    constexpr Chunk c = h_chunks.c[ci];
+    float (&d)[64] = acc[c.half];
     mbar_wait(&s.full[st], ph);
     wgmma_fence();
     const uint32_t bh = sbase + kOffRing + st * Smem::kStageBytes, bl = bh + kStepBytes * c.steps;
@@ -645,27 +677,157 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
                  bl + ks * kStepBytes, ks == 0 && c.first);
     });
     wgmma_commit();
-    if (!(c.first && c.half == 0)) {       // a layer's first chunk follows a drain: nothing to release
+    // a chunk that follows a drain has nothing to release: a tile's first chunk, and in the drained schedule
+    // (kTrain != 0) every layer's first chunk
+    if (kDrained ? !(c.first && c.half == 0) : ci != 0) {
       wgmma_wait<1>();                      // the previous chunk's wgmmas have retired
       if (lane == 0) mbar_arrive(&s.empty[prev_stage()]);
       __syncwarp();
     }
     if (++st == kStages) { st = 0; ph ^= 1; }
   };
-  auto issue_range = [&](auto c0tag, auto ntag, float (&d)[64]) SNB_INLINE {
-    static_for<decltype(ntag)::value>([&](auto i) SNB_INLINE {
-      issue_chunk(std::integral_constant<int, decltype(c0tag)::value + decltype(i)::value>{}, d);
-    });
+  auto issue_range = [&](auto c0tag, auto ntag) SNB_INLINE {
+    static_for<decltype(ntag)::value>([&](auto i) SNB_INLINE { issue(Int<decltype(c0tag)::value + decltype(i)::value>{}); });
   };
-  auto drain = [&]() {                      // all of a layer's wgmmas have retired
+  auto drain = [&]() {                      // all of the tile's wgmmas have retired
     wgmma_wait<0>();
     if (lane == 0) mbar_arrive(&s.empty[prev_stage()]);
     __syncwarp();
   };
 
-  float acc[2][64];              // a layer's two N = 128 halves
-  float sig[2] = {0.f, 0.f};     // sigma of rows r0, r0 + 8 (layer 7's epilogue -> the direction layer's)
+  // Epilogue block E(l, h, b) of trunk layer l (0..7) in inference: columns [128 h + 32 b, +32) of acc[h] -- bias,
+  // ReLU, hi/lo split -> hid K-block 4 h + b, which is one 32-K chunk of the next layer's A operand.  The sigma layer
+  // (kSigma) also accumulates the sigma head's partial sums, over its blocks in column order.
+  auto epi_block = [&](auto sigtag, auto htag, auto btag, int l, long long pt0) SNB_INLINE {
+    constexpr bool kSigma = decltype(sigtag)::value;
+    constexpr int h = decltype(htag)::value, b = decltype(btag)::value;
+    const float* bias = g_cst + l * kWidth;            // CL.b[l]
+    const float (&d)[64] = acc[h];
+    if (kSigma && h == 0 && b == 0) { sig[0] = 0.f; sig[1] = 0.f; }
+    static_for<4>([&](auto jtag) SNB_INLINE {
+      constexpr int j = 4 * b + decltype(jtag)::value;
+      const int col = h * kNh + 8 * j + 2 * tq;
+      const float2 bb = ldg_f2_here(bias + col);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        float x0 = d[4 * j + 2 * rr] + bb.x, x1 = d[4 * j + 2 * rr + 1] + bb.y;
+        uint32_t hi, lo;
+        if (!kSigma) {
+          // nobody needs the fp32 post-activation value: ReLU and the fp16 range guard ride on the converts
+          split_pair_relu<kBf16, kSplit>(x0, x1, hi, lo);
+        } else {
+          x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f);
+          const float2 ww = ldg_f2_here(g_cst + CL.sigma_w + col);
+          sig[rr] = fmaf(x0, ww.x, sig[rr]); sig[rr] = fmaf(x1, ww.y, sig[rr]);
+          split_pair<kBf16, kSplit, true>(x0, x1, hi, lo);
+        }
+        const uint32_t a = hid_thr + (h * 16 + j) * (kTile * 16) + rr * 128;   // canon_off(r0 + 8 rr, col)
+        st_shared_u32(a, hi);
+        if (kSplit) st_shared_u32(a + kHidPart, lo);
+      }
+    });
+  };
+  // the end of an epilogue (half): its hid blocks become visible to the next layer's wgmmas
+  auto epi_half_end = [&]() SNB_INLINE {
+    fence_proxy_async_smem();     // generic-proxy smem writes -> visible to the async proxy
+    wg_sync();
+  };
+  // sigma head (nerf.py:136) after the sigma layer's last epilogue block: the quad's four threads hold the row's columns
+  auto sigma_head = [&](long long pt0) SNB_INLINE {
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      float v = sig[rr];
+      v += __shfl_xor_sync(0xffffffffu, v, 1);
+      v += __shfl_xor_sync(0xffffffffu, v, 2);
+      sig[rr] = v + __ldg(g_cst + CL.sigma_b);
+      const long long pt = pt0 + 8 * rr;
+      if (p.sigma_only && tq == 0 && pt < p.n_points) p.out[pt] = sig[rr];
+    }
+  };
 
+  // direction layer: shifted softplus / ReLU, rgb head (nerf.py:142-146), the [r, g, b, sigma] rows
+  auto dir_epilogue = [&](const float (&d)[64], long long pt0) SNB_INLINE {
+    const float sh = new_activation ? 1.0f : 0.0f;   // shifted softplus: fold the -1 into the bias
+    float a[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int col = 8 * j + 2 * tq;
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(g_cst + CL.b[9] + col));
+      const float2 w0 = __ldg(reinterpret_cast<const float2*>(g_cst + CL.rgb_w + col));
+      const float2 w1 = __ldg(reinterpret_cast<const float2*>(g_cst + CL.rgb_w + kHalf + col));
+      const float2 w2 = __ldg(reinterpret_cast<const float2*>(g_cst + CL.rgb_w + 2 * kHalf + col));
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const long long pt = pt0 + 8 * rr;
+        float x0 = d[4 * j + 2 * rr] + (bb.x - sh), x1 = d[4 * j + 2 * rr + 1] + (bb.y - sh);
+        if (new_activation) { x0 = softplus_fast(x0); x1 = softplus_fast(x1); }
+        else { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        if (kTrain == 1 && pt < p.n_points) *reinterpret_cast<float2*>(p.save_g + pt * kHalf + col) = make_float2(x0, x1);
+        if (kTrain == 2 && pt < p.ppad)
+          *reinterpret_cast<uint32_t*>(p.a_g + a16_cell(pt, col >> 3, kHalf) + (col & 7) * 2) =
+              pt < p.n_points ? pack_half2_sat(x0, x1) : 0u;
+        a[rr][0] = fmaf(x1, w0.y, fmaf(x0, w0.x, a[rr][0]));
+        a[rr][1] = fmaf(x1, w1.y, fmaf(x0, w1.x, a[rr][1]));
+        a[rr][2] = fmaf(x1, w2.y, fmaf(x0, w2.x, a[rr][2]));
+      }
+    }
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      float c[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        float v = a[rr][k];
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        v += __ldg(g_cst + CL.rgb_b + k);
+        c[k] = new_activation ? widened_sigmoid_f(v) : sigmoid_f(v);
+      }
+      const long long pt = pt0 + 8 * rr;
+      if (tq == 0 && pt < p.n_points) reinterpret_cast<float4*>(p.out)[pt] = make_float4(c[0], c[1], c[2], sig[rr]);
+    }
+  };
+
+  // The epilogues run under the wgmmas: each epilogue block follows a chunk's issue and the wait<1> that retires the
+  // chunk before it, so one chunk stays queued on the tensor pipe while the block runs.  The only drain is at the end
+  // of a tile.  Per warpgroup (each reads and writes only its own rows of hid and enc):
+  //   1. E(l, h, b) reads acc[h]: every chunk of (l, h) has retired;
+  //   2. E(l, h, b) overwrites hid block 4 h + b: the chunk of (l, 1) that reads it has retired;
+  //   3. chunk k of (l + 1, h) reads hid block k only after the epilogue half that writes it has been fenced
+  //      (fence.proxy.async + warpgroup barrier);
+  //   4. the first wgmma of (l + 1, h) (accumulate = 0, writes acc[h]) follows every E(l, h, .) in program order.
+  //
+  // layer_body(L, l): the wgmmas of layer l, whose chunks follow layer L's schedule (layers 1-3, 5, 6 and 7 share
+  // layer 1's), interleaved with E(l - 1, 1, .) and E(l, 0, .).  On entry every chunk of layer l - 1 is issued and
+  // E(l - 1, 0, .) is fenced; on return every chunk of layer l is issued and E(l, 0, .) is fenced.
+  //   * E(l - 1, 1, b) follows (l, 0)'s chunk b: (l - 1, 1) has retired (rules 1, 2), and those chunks read only enc
+  //     and hid blocks 0-3 (rule 3);
+  //   * E(l, 0, b) follows (l, 1)'s chunk e + b + 1 (e = its enc chunks): (l, 0) and the (l, 1) chunk e + b that reads
+  //     hid block b have retired (rules 1, 2).
+  auto layer_body = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
+    constexpr int L = decltype(ltag)::value;
+    constexpr int c0 = chunk_index(L, 0), n0 = chunk_count(L, 0), c1 = chunk_index(L, 1), n1 = chunk_count(L, 1);
+    constexpr int e = enc_chunks(L);
+    static_for<4>([&](auto btag) SNB_INLINE {
+      issue(Int<c0 + decltype(btag)::value>{});
+      epi_block(std::false_type{}, Int<1>{}, btag, l - 1, pt0);
+    });
+    epi_half_end();
+    issue_range(Int<c0 + 4>{}, Int<n0 - 4>{});
+    issue_range(Int<c1>{}, Int<e + 1>{});
+    static_for<4>([&](auto btag) SNB_INLINE {
+      issue(Int<c1 + e + 1 + decltype(btag)::value>{});
+      epi_block(std::bool_constant<L == 7>{}, Int<0>{}, btag, l, pt0);
+    });
+    // (l, 0) and (l, 1)'s enc chunks, the last readers of this warpgroup's rows of the xyz encoding, have retired: the
+    // skip layer writes the direction encoding of the same rows over it
+    if (L == 4 && !p.sigma_only) encode_rows(Int<SNB_DIR_FREQS>{}, tile);
+    epi_half_end();
+    issue_range(Int<c1 + e + 5>{}, Int<n1 - e - 5>{});
+  };
+  // The training forward (kTrain != 0) keeps the drained schedule: one layer's wgmmas, the drain, then the layer's
+  // whole epilogue and one barrier.  With the blocked schedule it was slower (DESIGN.md §4.1): the global stores of
+  // the saved activations end up in front of one of a layer's two fences, and the registers that hold them push
+  // values out to local memory.
   // trunk epilogue of layer l (0..7): bias, ReLU, hi/lo split -> the next layer's A operand in shared memory.
   // L is the layer kind: 4 (skip layer: then writes the direction encoding), 7 (sigma head) or any other layer.
   auto trunk_epilogue = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
@@ -764,56 +926,10 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
     }
   };
 
-  // direction layer: shifted softplus / ReLU, rgb head (nerf.py:142-146), the [r, g, b, sigma] rows
-  auto dir_epilogue = [&](const float (&d)[64], long long pt0) SNB_INLINE {
-    const float sh = new_activation ? 1.0f : 0.0f;   // shifted softplus: fold the -1 into the bias
-    float a[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int col = 8 * j + 2 * tq;
-      const float2 bb = __ldg(reinterpret_cast<const float2*>(g_cst + CL.b[9] + col));
-      const float2 w0 = __ldg(reinterpret_cast<const float2*>(g_cst + CL.rgb_w + col));
-      const float2 w1 = __ldg(reinterpret_cast<const float2*>(g_cst + CL.rgb_w + kHalf + col));
-      const float2 w2 = __ldg(reinterpret_cast<const float2*>(g_cst + CL.rgb_w + 2 * kHalf + col));
-#pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        const long long pt = pt0 + 8 * rr;
-        float x0 = d[4 * j + 2 * rr] + (bb.x - sh), x1 = d[4 * j + 2 * rr + 1] + (bb.y - sh);
-        if (new_activation) { x0 = softplus_fast(x0); x1 = softplus_fast(x1); }
-        else { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-        if (kTrain == 1 && pt < p.n_points) *reinterpret_cast<float2*>(p.save_g + pt * kHalf + col) = make_float2(x0, x1);
-        if (kTrain == 2 && pt < p.ppad)
-          *reinterpret_cast<uint32_t*>(p.a_g + a16_cell(pt, col >> 3, kHalf) + (col & 7) * 2) =
-              pt < p.n_points ? pack_half2_sat(x0, x1) : 0u;
-        a[rr][0] = fmaf(x1, w0.y, fmaf(x0, w0.x, a[rr][0]));
-        a[rr][1] = fmaf(x1, w1.y, fmaf(x0, w1.x, a[rr][1]));
-        a[rr][2] = fmaf(x1, w2.y, fmaf(x0, w2.x, a[rr][2]));
-      }
-    }
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      float c[3];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        float v = a[rr][k];
-        v += __shfl_xor_sync(0xffffffffu, v, 1);
-        v += __shfl_xor_sync(0xffffffffu, v, 2);
-        v += __ldg(g_cst + CL.rgb_b + k);
-        c[k] = new_activation ? widened_sigmoid_f(v) : sigmoid_f(v);
-      }
-      const long long pt = pt0 + 8 * rr;
-      if (tq == 0 && pt < p.n_points) reinterpret_cast<float4*>(p.out)[pt] = make_float4(c[0], c[1], c[2], sig[rr]);
-    }
-  };
-
-  // one layer: its wgmmas in the schedule of layer L (layers 1-3, 5 and 6 share layer 1's), the drain, the epilogue.
-  // Each (layer, half) starts with a write-only wgmma (accumulate = 0), so no instruction writes an accumulator
-  // between a layer's first wgmma and its drain.
-  auto run_layer = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
+  auto drained_layer = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
     constexpr int L = decltype(ltag)::value;
-    issue_range(std::integral_constant<int, chunk_index(L, 0)>{}, std::integral_constant<int, chunk_count(L, 0)>{}, acc[0]);
-    if constexpr (L != 9)
-      issue_range(std::integral_constant<int, chunk_index(L, 1)>{}, std::integral_constant<int, chunk_count(L, 1)>{}, acc[1]);
+    issue_range(Int<chunk_index(L, 0)>{}, Int<chunk_count(L, 0)>{});
+    if constexpr (L != 9) issue_range(Int<chunk_index(L, 1)>{}, Int<chunk_count(L, 1)>{});
     drain();
     if constexpr (L == 9) dir_epilogue(acc[0], pt0);
     else trunk_epilogue(ltag, l, tile, pt0);
@@ -821,21 +937,68 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
   load_row(blockIdx.x);
   for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const long long pt0 = tile * kTile + r0;
-    // ---- xyz encoding of this warpgroup's 64 rows (the direction encoding follows layer 4)
-    encode_rows(std::integral_constant<int, SNB_XYZ_FREQS>{}, tile);
+    // ---- xyz encoding of this warpgroup's 64 rows (the direction encoding follows layer 4's enc chunks)
+    encode_rows(Int<SNB_XYZ_FREQS>{}, tile);
     fence_proxy_async_smem();
     wg_sync();
-    // layers 0..7, then the direction layer 9 (the bottleneck, 8, is folded into it); the plain hidden layers run
-    // as loops over one copy of the code, which keeps the kernel's instruction footprint down
-    run_layer(std::integral_constant<int, 0>{}, 0, tile, pt0);
+    if constexpr (kDrained) {
+      drained_layer(Int<0>{}, 0, tile, pt0);
 #pragma unroll 1
-    for (int l = 1; l < 4; ++l) run_layer(std::integral_constant<int, 1>{}, l, tile, pt0);
-    run_layer(std::integral_constant<int, 4>{}, 4, tile, pt0);
+      for (int l = 1; l < 4; ++l) drained_layer(Int<1>{}, l, tile, pt0);
+      drained_layer(Int<4>{}, 4, tile, pt0);
 #pragma unroll 1
-    for (int l = 5; l < 7; ++l) run_layer(std::integral_constant<int, 1>{}, l, tile, pt0);
-    run_layer(std::integral_constant<int, 7>{}, 7, tile, pt0);
-    load_row(tile + gridDim.x);   // the next tile's rays and depths, under this tile's last MMAs
-    if (!p.sigma_only) run_layer(std::integral_constant<int, 9>{}, 9, tile, pt0);   // sigma-only passes end with layer 7
+      for (int l = 5; l < 7; ++l) drained_layer(Int<1>{}, l, tile, pt0);
+      drained_layer(Int<7>{}, 7, tile, pt0);
+      load_row(tile + gridDim.x);
+      if (!p.sigma_only) drained_layer(Int<9>{}, 9, tile, pt0);
+    } else {
+      // layer 0 reads only enc, so its epilogue blocks have no hid hazard; E(0, 0, .) needs (0, 0) retired
+      issue_range(Int<chunk_index(0, 0)>{}, Int<chunk_count(0, 0)>{});
+      static_for<4>([&](auto btag) SNB_INLINE {
+        constexpr int b = decltype(btag)::value;
+        if constexpr (b < chunk_count(0, 1)) issue(Int<chunk_index(0, 1) + b>{});
+        epi_block(std::false_type{}, Int<0>{}, btag, 0, pt0);
+      });
+      epi_half_end();
+      // layers 1..7, then the direction layer 9 (the bottleneck, 8, is folded into it); the plain hidden layers run
+      // as loops over one copy of the code, which keeps the kernel's instruction footprint down.  No wgmma is in flight
+      // where a loop is entered or repeats: with an accumulator in flight there, ptxas serializes every wgmma of the
+      // kernel (C7514), since it may have to move the accumulator's registers at the merge.  Waiting for the last chunk
+      // of each layer costs the tensor pipe one restart per layer.
+      wgmma_wait<0>();
+#pragma unroll 1
+      for (int l = 1; l < 4; ++l) {
+        layer_body(Int<1>{}, l, tile, pt0);
+        wgmma_wait<0>();
+      }
+      layer_body(Int<4>{}, 4, tile, pt0);
+      wgmma_wait<0>();
+#pragma unroll 1
+      for (int l = 5; l < 7; ++l) {
+        layer_body(Int<1>{}, l, tile, pt0);
+        wgmma_wait<0>();
+      }
+      layer_body(Int<7>{}, 7, tile, pt0);
+      load_row(tile + gridDim.x);   // the next tile's rays and depths, under this tile's last MMAs
+      if (p.sigma_only) {           // sigma-only passes end with layer 7: E(7, 1, .) runs after the drain
+        drain();
+        static_for<4>([&](auto btag) SNB_INLINE { epi_block(std::true_type{}, Int<1>{}, btag, 7, pt0); });
+        sigma_head(pt0);
+        epi_half_end();
+        continue;
+      }
+      // the direction layer's chunks 0-3 read hid blocks 0-3 only; E(7, 1, .) runs under them
+      constexpr int c9 = chunk_index(9, 0);
+      static_for<4>([&](auto btag) SNB_INLINE {
+        issue(Int<c9 + decltype(btag)::value>{});
+        epi_block(std::true_type{}, Int<1>{}, btag, 7, pt0);
+      });
+      sigma_head(pt0);
+      epi_half_end();
+      issue_range(Int<c9 + 4>{}, Int<chunk_count(9, 0) - 4>{});
+      drain();
+      dir_epilogue(acc[0], pt0);
+    }
   }
 }
 
