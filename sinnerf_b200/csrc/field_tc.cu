@@ -14,7 +14,7 @@
 //     where the next layer's wgmmas read them as the A operand.  The consumers' layer schedule is unrolled at
 //     compile time: chunk sources, offsets and accumulators are constants, and the first wgmma of a (layer, half)
 //     writes its accumulator without reading it (scale-d = 0).  The epilogue runs in 32-column blocks, each one
-//     K chunk of the next layer's input, interleaved with the wgmmas still in flight (see layer_body);
+//     K chunk of the next layer's input, interleaved with the wgmmas still in flight (see trunk_layer);
 //   * weights stream from L2 through a shared-memory ring of chunks (128 output rows x 32 K x {hi, lo};
 //     4 stages in the split modes, 18 in bf16) with cp.async.bulk (1-D TMA) + mbarrier complete_tx, issued
 //     by one producer thread that runs ahead over all of the CTA's tiles; the consumers only wait on
@@ -333,10 +333,9 @@ __device__ __forceinline__ void sincos_fast(float x, float* sn, float* cs) {
   *cs = __cosf(r);
 }
 // ------------------------------------------------------------------ pack kernel
-using ParamPtrsTc = ParamPtrs;
 
 // W'[n][k] = sum_j Wd[n][j] Wf[j][k],  b'[n] = bd[n] + sum_j Wd[n][j] bf[j]   (double accumulation)
-__global__ void fuse_bottleneck_kernel(ParamPtrsTc pp, float* fused, const PackedHeader* hdr, int only_if_dirty) {
+__global__ void fuse_bottleneck_kernel(ParamPtrs pp, float* fused, const PackedHeader* hdr, int only_if_dirty) {
   if (only_if_dirty && !hdr->dirty) return;
   const float* Wd = pp.p[18];   // (128, 283)
   const float* Wf = pp.p[16];   // (256, 256)
@@ -352,7 +351,7 @@ __global__ void fuse_bottleneck_kernel(ParamPtrsTc pp, float* fused, const Packe
 }
 
 template <bool kBf16, bool kSplit>
-__global__ void pack_tc_kernel(ParamPtrsTc pp, int precision, int new_activation, unsigned char* image, int only_if_dirty) {
+__global__ void pack_tc_kernel(ParamPtrs pp, int precision, int new_activation, unsigned char* image, int only_if_dirty) {
   constexpr ConstLayout CL = make_const_layout();
   const ChunkTable& tab = c_chunks;
   PackedHeader* hdr = reinterpret_cast<PackedHeader*>(image);
@@ -413,7 +412,7 @@ __global__ void pack_tc_kernel(ParamPtrsTc pp, int precision, int new_activation
 
 int launch_pack_tc(const float* const* params, int precision, int new_activation, void* image, int only_if_dirty,
                    cudaStream_t st) {
-  ParamPtrsTc pp;
+  ParamPtrs pp;
   for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) pp.p[i] = params[i];
   unsigned char* img = reinterpret_cast<unsigned char*>(image);
   if (precision < SNB_PREC_F16X3 || precision > SNB_PREC_BF16)
@@ -469,9 +468,6 @@ struct TcParams {
   uint32_t* a_mask;        // (8, 8, Ppad)
   long long ppad;
 };
-
-// canonical (SWIZZLE_NONE, K-major) byte offset of element (row, k) in a [k8][128 rows][8] block
-__device__ __forceinline__ uint32_t canon_off(int row, int k) { return (uint32_t)(k >> 3) * (kTile * 16) + row * 16 + (k & 7) * 2; }
 
 // kTrain: 0 = inference, 1 = training forward keeping fp32 row-major activations (snb_field_forward_train),
 //         2 = training forward keeping fp16 activations in the T32 layout + ReLU mask words (act16.cuh)
@@ -534,7 +530,9 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
   constexpr uint32_t kOffRing = offsetof(Smem, ring), kOffHid = offsetof(Smem, hid), kOffEnc = offsetof(Smem, enc);
   const uint32_t sbase = smem_u32(&s);
   const uint32_t a_wg = sbase + wgi * 64 * 16;              // this warpgroup's A rows (+ kOffHid / kOffEnc)
-  const uint32_t hid_thr = sbase + kOffHid + r0 * 16 + tq * 4;   // canon_off(r0, 2 tq): this thread's first epilogue word
+  // this thread's first epilogue word, (row r0, column 2 tq): the canonical [k8][row][8] layout puts (row, k) at byte
+  // (k >> 3) * (kTile * 16) + row * 16 + (k & 7) * 2
+  const uint32_t hid_thr = sbase + kOffHid + r0 * 16 + tq * 4;
   // encodings: the tile row and the half of its channels this thread computes (all 128 threads of a warpgroup)
   const int er = wgi * 64 + (tid & 63), epart = (tid >> 6) & 1;
 
@@ -649,7 +647,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
     }
   };
 
-  constexpr bool kDrained = kTrain != 0;   // the training forward keeps the drained schedule (drained_layer)
+  constexpr bool kDrained = kTrain != 0;   // the training forward keeps the drained schedule (trunk_layer)
   float acc[2][64];              // a layer's two N = 128 halves
   float sig[2] = {0.f, 0.f};     // sigma of rows r0, r0 + 8 (layer 7's epilogue -> the direction layer's)
 
@@ -695,37 +693,60 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
     __syncwarp();
   };
 
-  // Epilogue block E(l, h, b) of trunk layer l (0..7) in inference: columns [128 h + 32 b, +32) of acc[h] -- bias,
-  // ReLU, hi/lo split -> hid K-block 4 h + b, which is one 32-K chunk of the next layer's A operand.  The sigma layer
-  // (kSigma) also accumulates the sigma head's partial sums, over its blocks in column order.
+  // Epilogue block E(l, h, b) of trunk layer l (0..7): columns [128 h + 32 b, +32) of acc[h] -- bias, ReLU, hi/lo
+  // split -> hid K-block 4 h + b, which is one 32-K chunk of the next layer's A operand.  The sigma layer (kSigma) also
+  // accumulates the sigma head's partial sums, over its blocks in column order.  The training forward saves the
+  // post-activation values: kTrain == 1 stores them as fp32 rows; for kTrain == 2 the block returns its fp16 words and
+  // its ReLU mask word (one 32-column block is one word) for the caller to store after the epilogue's barrier.
+  struct Block16 { uint32_t h16[4][2], mask[2]; };
   auto epi_block = [&](auto sigtag, auto htag, auto btag, int l, long long pt0) SNB_INLINE {
     constexpr bool kSigma = decltype(sigtag)::value;
     constexpr int h = decltype(htag)::value, b = decltype(btag)::value;
     const float* bias = g_cst + l * kWidth;            // CL.b[l]
     const float (&d)[64] = acc[h];
+    Block16 k16{};
     if (kSigma && h == 0 && b == 0) { sig[0] = 0.f; sig[1] = 0.f; }
     static_for<4>([&](auto jtag) SNB_INLINE {
-      constexpr int j = 4 * b + decltype(jtag)::value;
+      constexpr int jj = decltype(jtag)::value, j = 4 * b + jj;
       const int col = h * kNh + 8 * j + 2 * tq;
       const float2 bb = ldg_f2_here(bias + col);
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         float x0 = d[4 * j + 2 * rr] + bb.x, x1 = d[4 * j + 2 * rr + 1] + bb.y;
         uint32_t hi, lo;
-        if (!kSigma) {
+        if (kTrain == 0 && !kSigma) {
           // nobody needs the fp32 post-activation value: ReLU and the fp16 range guard ride on the converts
           split_pair_relu<kBf16, kSplit>(x0, x1, hi, lo);
         } else {
           x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f);
-          const float2 ww = ldg_f2_here(g_cst + CL.sigma_w + col);
-          sig[rr] = fmaf(x0, ww.x, sig[rr]); sig[rr] = fmaf(x1, ww.y, sig[rr]);
+          if (kSigma) {
+            const float2 ww = ldg_f2_here(g_cst + CL.sigma_w + col);
+            sig[rr] = fmaf(x0, ww.x, sig[rr]); sig[rr] = fmaf(x1, ww.y, sig[rr]);
+          }
           split_pair<kBf16, kSplit, true>(x0, x1, hi, lo);
+          const long long pt = pt0 + 8 * rr;
+          if (kTrain == 1 && pt < p.n_points)
+            *reinterpret_cast<float2*>(p.save_h + ((size_t)l * p.n_points + pt) * kWidth + col) = make_float2(x0, x1);
+          if (kTrain == 2) {
+            // fp16 modes: the hi word of the split IS rn_fp16(value) (saturated); bf16 modes convert separately
+            k16.h16[jj][rr] = kBf16 ? pack_half2_sat(x0, x1) : hi;
+            k16.mask[rr] |= ((x0 > 0.f ? 1u : 0u) << (col & 31)) | ((x1 > 0.f ? 1u : 0u) << ((col & 31) + 1));
+          }
         }
-        const uint32_t a = hid_thr + (h * 16 + j) * (kTile * 16) + rr * 128;   // canon_off(r0 + 8 rr, col)
+        const uint32_t a = hid_thr + (h * 16 + j) * (kTile * 16) + rr * 128;   // (row r0 + 8 rr, column col)
         st_shared_u32(a, hi);
         if (kSplit) st_shared_u32(a + kHidPart, lo);
       }
     });
+    if (kTrain == 2) {
+      // the quad's four threads hold the block's 32 ReLU bits of each row
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        k16.mask[rr] |= __shfl_xor_sync(0xffffffffu, k16.mask[rr], 1);
+        k16.mask[rr] |= __shfl_xor_sync(0xffffffffu, k16.mask[rr], 2);
+      }
+    }
+    return k16;
   };
   // the end of an epilogue (half): its hid blocks become visible to the next layer's wgmmas
   auto epi_half_end = [&]() SNB_INLINE {
@@ -787,123 +808,21 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
     }
   };
 
-  // The epilogues run under the wgmmas: each epilogue block follows a chunk's issue and the wait<1> that retires the
-  // chunk before it, so one chunk stays queued on the tensor pipe while the block runs.  The only drain is at the end
-  // of a tile.  Per warpgroup (each reads and writes only its own rows of hid and enc):
-  //   1. E(l, h, b) reads acc[h]: every chunk of (l, h) has retired;
-  //   2. E(l, h, b) overwrites hid block 4 h + b: the chunk of (l, 1) that reads it has retired;
-  //   3. chunk k of (l + 1, h) reads hid block k only after the epilogue half that writes it has been fenced
-  //      (fence.proxy.async + warpgroup barrier);
-  //   4. the first wgmma of (l + 1, h) (accumulate = 0, writes acc[h]) follows every E(l, h, .) in program order.
-  //
-  // layer_body(L, l): the wgmmas of layer l, whose chunks follow layer L's schedule (layers 1-3, 5, 6 and 7 share
-  // layer 1's), interleaved with E(l - 1, 1, .) and E(l, 0, .).  On entry every chunk of layer l - 1 is issued and
-  // E(l - 1, 0, .) is fenced; on return every chunk of layer l is issued and E(l, 0, .) is fenced.
-  //   * E(l - 1, 1, b) follows (l, 0)'s chunk b: (l - 1, 1) has retired (rules 1, 2), and those chunks read only enc
-  //     and hid blocks 0-3 (rule 3);
-  //   * E(l, 0, b) follows (l, 1)'s chunk e + b + 1 (e = its enc chunks): (l, 0) and the (l, 1) chunk e + b that reads
-  //     hid block b have retired (rules 1, 2).
-  auto layer_body = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
-    constexpr int L = decltype(ltag)::value;
-    constexpr int c0 = chunk_index(L, 0), n0 = chunk_count(L, 0), c1 = chunk_index(L, 1), n1 = chunk_count(L, 1);
-    constexpr int e = enc_chunks(L);
-    static_for<4>([&](auto btag) SNB_INLINE {
-      issue(Int<c0 + decltype(btag)::value>{});
-      epi_block(std::false_type{}, Int<1>{}, btag, l - 1, pt0);
-    });
-    epi_half_end();
-    issue_range(Int<c0 + 4>{}, Int<n0 - 4>{});
-    issue_range(Int<c1>{}, Int<e + 1>{});
-    static_for<4>([&](auto btag) SNB_INLINE {
-      issue(Int<c1 + e + 1 + decltype(btag)::value>{});
-      epi_block(std::bool_constant<L == 7>{}, Int<0>{}, btag, l, pt0);
-    });
-    // (l, 0) and (l, 1)'s enc chunks, the last readers of this warpgroup's rows of the xyz encoding, have retired: the
-    // skip layer writes the direction encoding of the same rows over it
-    if (L == 4 && !p.sigma_only) encode_rows(Int<SNB_DIR_FREQS>{}, tile);
-    epi_half_end();
-    issue_range(Int<c1 + e + 5>{}, Int<n1 - e - 5>{});
-  };
-  // The training forward (kTrain != 0) keeps the drained schedule: one layer's wgmmas, the drain, then the layer's
-  // whole epilogue and one barrier.  With the blocked schedule it was slower (DESIGN.md §4.1): the global stores of
-  // the saved activations end up in front of one of a layer's two fences, and the registers that hold them push
-  // values out to local memory.
-  // trunk epilogue of layer l (0..7): bias, ReLU, hi/lo split -> the next layer's A operand in shared memory.
-  // L is the layer kind: 4 (skip layer: then writes the direction encoding), 7 (sigma head) or any other layer.
+  // The drained trunk epilogue of layer l: all eight blocks in drain order, the sigma head, the skip layer's direction
+  // encoding and one barrier.  kTrain == 2 keeps the fp16 activation words and ReLU mask words in registers and stores
+  // them to global memory after that barrier; stored inside it, they made the epilogue's `fence.proxy.async`
+  // (MEMBAR.ALL.CTA) wait for their completion in every layer.
   auto trunk_epilogue = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
     constexpr int L = decltype(ltag)::value;
-    constexpr bool kSigma = L == 7;
-    const float* bias = g_cst + l * kWidth;            // CL.b[l]
-    // kTrain == 2: the fp16 activation words and ReLU mask words are kept in registers and stored to global memory
-    // after the barrier that ends the epilogue; stored inside it, they made the epilogue's `fence.proxy.async`
-    // (MEMBAR.ALL.CTA) wait for their completion in every layer
-    uint32_t h16v[2][16][2], mwv[2][4][2];
-    if (kSigma) { sig[0] = 0.f; sig[1] = 0.f; }
+    Block16 k16[2][4];
     static_for<2>([&](auto htag) SNB_INLINE {
-      constexpr int h = decltype(htag)::value;
-      float (&d)[64] = acc[h];
-      uint32_t mw[2] = {0u, 0u};
-      static_for<16>([&](auto jtag) SNB_INLINE {
-        constexpr int j = decltype(jtag)::value;
-        const int col = h * kNh + 8 * j + 2 * tq;
-        const float2 bb = ldg_f2_here(bias + col);
-#pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          const long long pt = pt0 + 8 * rr;
-          float x0 = d[4 * j + 2 * rr] + bb.x, x1 = d[4 * j + 2 * rr + 1] + bb.y;
-          uint32_t hi, lo;
-          if (kTrain == 0 && !kSigma) {
-            // nobody needs the fp32 post-activation value: ReLU and the fp16 range guard ride on the converts
-            split_pair_relu<kBf16, kSplit>(x0, x1, hi, lo);
-          } else {
-            x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f);
-            if (kSigma) {
-              const float2 ww = ldg_f2_here(g_cst + CL.sigma_w + col);
-              sig[rr] = fmaf(x0, ww.x, sig[rr]); sig[rr] = fmaf(x1, ww.y, sig[rr]);
-            }
-            split_pair<kBf16, kSplit, true>(x0, x1, hi, lo);
-            if (kTrain == 1 && pt < p.n_points)
-              *reinterpret_cast<float2*>(p.save_h + ((size_t)l * p.n_points + pt) * kWidth + col) = make_float2(x0, x1);
-            if (kTrain == 2) {
-              // fp16 modes: the hi word of the split IS rn_fp16(value) (saturated); bf16 modes convert separately
-              h16v[h][j][rr] = kBf16 ? pack_half2_sat(x0, x1) : hi;
-              mw[rr] |= ((x0 > 0.f ? 1u : 0u) << (col & 31)) | ((x1 > 0.f ? 1u : 0u) << ((col & 31) + 1));
-            }
-          }
-          const uint32_t a = hid_thr + (h * 16 + j) * (kTile * 16) + rr * 128;   // canon_off(r0 + 8 rr, col)
-          st_shared_u32(a, hi);
-          if (kSplit) st_shared_u32(a + kHidPart, lo);
-        }
-        if (kTrain == 2 && (j & 3) == 3) {
-          // a 32-column group is complete: the quad's four threads hold its 32 ReLU bits of each row
-#pragma unroll
-          for (int rr = 0; rr < 2; ++rr) {
-            uint32_t w = mw[rr];
-            w |= __shfl_xor_sync(0xffffffffu, w, 1);
-            w |= __shfl_xor_sync(0xffffffffu, w, 2);
-            mwv[h][j / 4][rr] = w;
-            mw[rr] = 0u;
-          }
-        }
+      static_for<4>([&](auto btag) SNB_INLINE {
+        k16[decltype(htag)::value][decltype(btag)::value] = epi_block(std::bool_constant<L == 7>{}, htag, btag, l, pt0);
       });
     });
-    if (kSigma) {
-      // sigma head (nerf.py:136): the quad's four threads hold the row's columns
-#pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        float v = sig[rr];
-        v += __shfl_xor_sync(0xffffffffu, v, 1);
-        v += __shfl_xor_sync(0xffffffffu, v, 2);
-        sig[rr] = v + __ldg(g_cst + CL.sigma_b);
-        const long long pt = pt0 + 8 * rr;
-        if (p.sigma_only && tq == 0 && pt < p.n_points) p.out[pt] = sig[rr];
-      }
-    }
-    // this warpgroup's layer-4 wgmmas, the last readers of its rows of the xyz encoding, have retired: it writes
-    // the direction encoding of the same rows over it
-    if (L == 4 && !p.sigma_only) encode_rows(std::integral_constant<int, SNB_DIR_FREQS>{}, tile);
-    fence_proxy_async_smem();     // generic-proxy smem writes -> visible to the next layer's wgmmas
-    wg_sync();
+    if (L == 7) sigma_head(pt0);
+    if (L == 4 && !p.sigma_only) encode_rows(Int<SNB_DIR_FREQS>{}, tile);
+    epi_half_end();
     if (kTrain == 2) {
       unsigned char* hb = p.a_h + (size_t)l * (size_t)p.ppad * (kWidth * 2);
 #pragma unroll
@@ -916,24 +835,113 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             const int col = h * kNh + 8 * j + 2 * tq;
-            *reinterpret_cast<uint32_t*>(hb + a16_cell(pt, col >> 3, kWidth) + (col & 7) * 2) = live ? h16v[h][j][rr] : 0u;
+            *reinterpret_cast<uint32_t*>(hb + a16_cell(pt, col >> 3, kWidth) + (col & 7) * 2) =
+                live ? k16[h][j / 4].h16[j % 4][rr] : 0u;
           }
 #pragma unroll
-          for (int g = 0; g < 4; ++g)
-            if (tq == 0) p.a_mask[a16_mask_index(l, h * 4 + g, pt, p.ppad)] = live ? mwv[h][g][rr] : 0u;
+          for (int b = 0; b < 4; ++b)
+            if (tq == 0) p.a_mask[a16_mask_index(l, h * 4 + b, pt, p.ppad)] = live ? k16[h][b].mask[rr] : 0u;
         }
       }
     }
   };
 
-  auto drained_layer = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
+  // Two schedules, selected at compile time.  Inference (the render path and the embedded entry) runs the epilogues
+  // under the wgmmas: each epilogue block follows a chunk's issue and the wait<1> that retires the chunk before it, so
+  // one chunk stays queued on the tensor pipe while the block runs.  The training forward (kDrained) runs a layer's
+  // wgmmas, drains them, then runs the layer's whole epilogue under one barrier: with the blocked schedule it was
+  // slower (DESIGN.md §4.1), since the global stores of the saved activations end up in front of one of a layer's two
+  // fences and the registers that hold them push values out to local memory.
+  //
+  // Blocked, per warpgroup (each reads and writes only its own rows of hid and enc):
+  //   1. E(l, h, b) reads acc[h]: every chunk of (l, h) has retired;
+  //   2. E(l, h, b) overwrites hid block 4 h + b: the chunk of (l, 1) that reads it has retired;
+  //   3. chunk k of (l + 1, h) reads hid block k only after the epilogue half that writes it has been fenced
+  //      (fence.proxy.async + warpgroup barrier);
+  //   4. the first wgmma of (l + 1, h) (accumulate = 0, writes acc[h]) follows every E(l, h, .) in program order.
+  //
+  // trunk_layer(L, l): the wgmmas of trunk layer l, whose chunks follow layer L's schedule (layers 1-3, 5 and 6 share
+  // layer 1's), and the epilogue blocks the schedule places under them.  Blocked, layer l > 0 interleaves them with
+  // E(l - 1, 1, .) and E(l, 0, .).  On entry every chunk of layer l - 1 is issued and E(l - 1, 0, .) is fenced; on
+  // return every chunk of layer l is issued and E(l, 0, .) is fenced.
+  //   * E(l - 1, 1, b) follows (l, 0)'s chunk b: (l - 1, 1) has retired (rules 1, 2), and those chunks read only enc
+  //     and hid blocks 0-3 (rule 3);
+  //   * E(l, 0, b) follows (l, 1)'s chunk e + b + 1 (e = its enc chunks): (l, 0) and the (l, 1) chunk e + b that reads
+  //     hid block b have retired (rules 1, 2);
+  //   * layer 0 reads only enc and its half 1 holds only enc chunks, so its blocks have no hid hazard: E(0, 0, .)
+  //     needs only (0, 0) retired.
+  // No wgmma is in flight where a loop over layers is entered or repeats: with an accumulator in flight there, ptxas
+  // serializes every wgmma of the kernel (C7514), since it may have to move the accumulator's registers at the merge.
+  // So every blocked layer but 7 ends by waiting for its last chunk, which costs the tensor pipe one restart per layer.
+  //
+  // The skip layer (L = 4) writes the direction encoding over this warpgroup's rows of the xyz encoding once (4, 0)
+  // and (4, 1)'s enc chunks, its last readers, have retired.
+  auto trunk_layer = [&](auto ltag, int l, long long tile, long long pt0) SNB_INLINE {
     constexpr int L = decltype(ltag)::value;
-    issue_range(Int<chunk_index(L, 0)>{}, Int<chunk_count(L, 0)>{});
-    if constexpr (L != 9) issue_range(Int<chunk_index(L, 1)>{}, Int<chunk_count(L, 1)>{});
-    drain();
-    if constexpr (L == 9) dir_epilogue(acc[0], pt0);
-    else trunk_epilogue(ltag, l, tile, pt0);
+    constexpr int c0 = chunk_index(L, 0), n0 = chunk_count(L, 0), c1 = chunk_index(L, 1), n1 = chunk_count(L, 1);
+    constexpr int e = enc_chunks(L);
+    if constexpr (kDrained) {
+      issue_range(Int<c0>{}, Int<n0>{});
+      issue_range(Int<c1>{}, Int<n1>{});
+      drain();
+      trunk_epilogue(ltag, l, tile, pt0);
+    } else if constexpr (L == 0) {
+      issue_range(Int<c0>{}, Int<n0>{});
+      static_for<4>([&](auto btag) SNB_INLINE {
+        constexpr int b = decltype(btag)::value;
+        if constexpr (b < n1) issue(Int<c1 + b>{});
+        epi_block(std::false_type{}, Int<0>{}, btag, 0, pt0);
+      });
+      epi_half_end();
+      wgmma_wait<0>();
+    } else {
+      static_for<4>([&](auto btag) SNB_INLINE {
+        issue(Int<c0 + decltype(btag)::value>{});
+        epi_block(std::false_type{}, Int<1>{}, btag, l - 1, pt0);
+      });
+      epi_half_end();
+      issue_range(Int<c0 + 4>{}, Int<n0 - 4>{});
+      issue_range(Int<c1>{}, Int<e + 1>{});
+      static_for<4>([&](auto btag) SNB_INLINE {
+        issue(Int<c1 + e + 1 + decltype(btag)::value>{});
+        epi_block(std::bool_constant<L == 7>{}, Int<0>{}, btag, l, pt0);
+      });
+      if (L == 4 && !p.sigma_only) encode_rows(Int<SNB_DIR_FREQS>{}, tile);
+      epi_half_end();
+      issue_range(Int<c1 + e + 5>{}, Int<n1 - e - 5>{});
+      if constexpr (L != 7) wgmma_wait<0>();
+    }
   };
+  // The end of a tile: the direction layer 9 (the bottleneck, 8, is folded into it) and its epilogue.  Blocked,
+  // E(7, 1, .) runs under the direction layer's chunks 0-3, which read hid blocks 0-3 only; sigma-only passes end with
+  // layer 7, so there E(7, 1, .) runs after the drain.
+  auto tile_end = [&](long long tile, long long pt0) SNB_INLINE {
+    constexpr int c9 = chunk_index(9, 0), n9 = chunk_count(9, 0);
+    load_row(tile + gridDim.x);   // the next tile's rays and depths, under this tile's last MMAs
+    if (p.sigma_only) {
+      if constexpr (!kDrained) {
+        drain();
+        static_for<4>([&](auto btag) SNB_INLINE { epi_block(std::true_type{}, Int<1>{}, btag, 7, pt0); });
+        sigma_head(pt0);
+        epi_half_end();
+      }
+      return;
+    }
+    if constexpr (kDrained) {
+      issue_range(Int<c9>{}, Int<n9>{});
+    } else {
+      static_for<4>([&](auto btag) SNB_INLINE {
+        issue(Int<c9 + decltype(btag)::value>{});
+        epi_block(std::true_type{}, Int<1>{}, btag, 7, pt0);
+      });
+      sigma_head(pt0);
+      epi_half_end();
+      issue_range(Int<c9 + 4>{}, Int<n9 - 4>{});
+    }
+    drain();
+    dir_epilogue(acc[0], pt0);
+  };
+
   load_row(blockIdx.x);
   for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const long long pt0 = tile * kTile + r0;
@@ -941,64 +949,15 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(TcParams p) {
     encode_rows(Int<SNB_XYZ_FREQS>{}, tile);
     fence_proxy_async_smem();
     wg_sync();
-    if constexpr (kDrained) {
-      drained_layer(Int<0>{}, 0, tile, pt0);
+    // the plain hidden layers run as loops over one copy of the code, which keeps the kernel's instruction footprint down
+    trunk_layer(Int<0>{}, 0, tile, pt0);
 #pragma unroll 1
-      for (int l = 1; l < 4; ++l) drained_layer(Int<1>{}, l, tile, pt0);
-      drained_layer(Int<4>{}, 4, tile, pt0);
+    for (int l = 1; l < 4; ++l) trunk_layer(Int<1>{}, l, tile, pt0);
+    trunk_layer(Int<4>{}, 4, tile, pt0);
 #pragma unroll 1
-      for (int l = 5; l < 7; ++l) drained_layer(Int<1>{}, l, tile, pt0);
-      drained_layer(Int<7>{}, 7, tile, pt0);
-      load_row(tile + gridDim.x);
-      if (!p.sigma_only) drained_layer(Int<9>{}, 9, tile, pt0);
-    } else {
-      // layer 0 reads only enc, so its epilogue blocks have no hid hazard; E(0, 0, .) needs (0, 0) retired
-      issue_range(Int<chunk_index(0, 0)>{}, Int<chunk_count(0, 0)>{});
-      static_for<4>([&](auto btag) SNB_INLINE {
-        constexpr int b = decltype(btag)::value;
-        if constexpr (b < chunk_count(0, 1)) issue(Int<chunk_index(0, 1) + b>{});
-        epi_block(std::false_type{}, Int<0>{}, btag, 0, pt0);
-      });
-      epi_half_end();
-      // layers 1..7, then the direction layer 9 (the bottleneck, 8, is folded into it); the plain hidden layers run
-      // as loops over one copy of the code, which keeps the kernel's instruction footprint down.  No wgmma is in flight
-      // where a loop is entered or repeats: with an accumulator in flight there, ptxas serializes every wgmma of the
-      // kernel (C7514), since it may have to move the accumulator's registers at the merge.  Waiting for the last chunk
-      // of each layer costs the tensor pipe one restart per layer.
-      wgmma_wait<0>();
-#pragma unroll 1
-      for (int l = 1; l < 4; ++l) {
-        layer_body(Int<1>{}, l, tile, pt0);
-        wgmma_wait<0>();
-      }
-      layer_body(Int<4>{}, 4, tile, pt0);
-      wgmma_wait<0>();
-#pragma unroll 1
-      for (int l = 5; l < 7; ++l) {
-        layer_body(Int<1>{}, l, tile, pt0);
-        wgmma_wait<0>();
-      }
-      layer_body(Int<7>{}, 7, tile, pt0);
-      load_row(tile + gridDim.x);   // the next tile's rays and depths, under this tile's last MMAs
-      if (p.sigma_only) {           // sigma-only passes end with layer 7: E(7, 1, .) runs after the drain
-        drain();
-        static_for<4>([&](auto btag) SNB_INLINE { epi_block(std::true_type{}, Int<1>{}, btag, 7, pt0); });
-        sigma_head(pt0);
-        epi_half_end();
-        continue;
-      }
-      // the direction layer's chunks 0-3 read hid blocks 0-3 only; E(7, 1, .) runs under them
-      constexpr int c9 = chunk_index(9, 0);
-      static_for<4>([&](auto btag) SNB_INLINE {
-        issue(Int<c9 + decltype(btag)::value>{});
-        epi_block(std::true_type{}, Int<1>{}, btag, 7, pt0);
-      });
-      sigma_head(pt0);
-      epi_half_end();
-      issue_range(Int<c9 + 4>{}, Int<chunk_count(9, 0) - 4>{});
-      drain();
-      dir_epilogue(acc[0], pt0);
-    }
+    for (int l = 5; l < 7; ++l) trunk_layer(Int<1>{}, l, tile, pt0);
+    trunk_layer(Int<7>{}, 7, tile, pt0);
+    tile_end(tile, pt0);
   }
 }
 
@@ -1017,12 +976,12 @@ static int launch_tc(const TcParams& p, cudaStream_t st) {
   return check_launch("field_tc_kernel");
 }
 
-template <bool kEmbedded>
+template <bool kEmbedded, int kTrain = 0>
 static int dispatch_tc(int precision, const TcParams& p, cudaStream_t st) {
   switch (precision) {
-    case SNB_PREC_F16X3: return launch_tc<false, true, kEmbedded>(p, st);
-    case SNB_PREC_BF16X3: return launch_tc<true, true, kEmbedded>(p, st);
-    case SNB_PREC_BF16: return launch_tc<true, false, kEmbedded>(p, st);
+    case SNB_PREC_F16X3: return launch_tc<false, true, kEmbedded, kTrain>(p, st);
+    case SNB_PREC_BF16X3: return launch_tc<true, true, kEmbedded, kTrain>(p, st);
+    case SNB_PREC_BF16: return launch_tc<true, false, kEmbedded, kTrain>(p, st);
   }
   return fail(SNB_ERR_INVALID, "precision %d is not a tensor-core mode", precision);
 }
@@ -1047,12 +1006,7 @@ int field_forward_train_tc(const void* packed, int precision, const float* rays,
   p.n_points = (long long)n_rays * n_samples;
   p.out = raw;
   p.save_enc = save_enc; p.save_dir = save_dir; p.save_h = save_h; p.save_g = save_g;
-  switch (precision) {
-    case SNB_PREC_F16X3: return launch_tc<false, true, false, 1>(p, st);
-    case SNB_PREC_BF16X3: return launch_tc<true, true, false, 1>(p, st);
-    case SNB_PREC_BF16: return launch_tc<true, false, false, 1>(p, st);
-  }
-  return fail(SNB_ERR_INVALID, "precision %d is not a tensor-core mode", precision);
+  return dispatch_tc<false, 1>(precision, p, st);
 }
 
 // training forward with 16-bit activation storage (act16.cuh): `act16` = one buffer of make_act16_layout(P).total bytes
@@ -1068,12 +1022,7 @@ int field_forward_train16_tc(const void* packed, int precision, const float* ray
   p.a_enc = b + L.enc; p.a_dir = b + L.dir; p.a_h = b + L.h[0]; p.a_g = b + L.g;
   p.a_mask = reinterpret_cast<uint32_t*>(b + L.mask);
   p.ppad = a16_pad(p.n_points);
-  switch (precision) {
-    case SNB_PREC_F16X3: return launch_tc<false, true, false, 2>(p, st);
-    case SNB_PREC_BF16X3: return launch_tc<true, true, false, 2>(p, st);
-    case SNB_PREC_BF16: return launch_tc<true, false, false, 2>(p, st);
-  }
-  return fail(SNB_ERR_INVALID, "precision %d is not a tensor-core mode", precision);
+  return dispatch_tc<false, 2>(precision, p, st);
 }
 
 int mlp_forward_tc(const void* packed, int precision, const float* x, int64_t x_stride, int64_t n_points,

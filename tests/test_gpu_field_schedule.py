@@ -31,7 +31,9 @@ def packed_image(precision):
 
 
 def assert_rows_equal(shared, base, what):
-    bad = (shared.view(torch.int32) != base.view(torch.int32)).reshape(-1, base.shape[-1]).any(dim=1)   # per point
+    if base.dtype == torch.float32:   # compare the bits
+        shared, base = shared.view(torch.int32), base.view(torch.int32)
+    bad = (shared != base).reshape(-1, base.shape[-1]).any(dim=1)   # per point
     assert not bool(bad.any()), f"{what}: {int(bad.sum())} of {bad.numel()} points differ, first at {int(bad.nonzero()[0])}"
 
 
@@ -87,3 +89,56 @@ def test_embedded_rows_independent_of_tile_offset(precision, sigma_only):
     assert torch.isfinite(base).all()
     for k in (1, 37, 127):
         assert_rows_equal(run(x_all[127 - k:].contiguous())[k:], base, f"{precision} sigma_only={sigma_only} k={k}")
+
+
+@pytest.mark.parametrize("precision", TENSOR_MODES)
+def test_train16_saves_the_fp32_activations_rounded(precision):
+    """The two training forwards run the same epilogue arithmetic and differ only in what they save.
+    snb_field_forward_train16's raw output is the same bits as snb_field_forward_train's; each of its fp16 T32 cells is
+    the fp32 activation the other saves, saturated and rounded to fp16; its ReLU mask bits are the signs of the saved
+    layer outputs.  52 800 points leave the last tile partial; the padded points must be zero."""
+    from sinnerf_b200 import _lib, synthetic
+    lib = _lib.load()
+    prec = _lib.precision_id(precision)
+    img = packed_image(precision)
+    rays = synthetic.frame_rays("lego", seed=0)[:N_RAYS].to(DEV).contiguous()
+    g = torch.Generator(device=DEV).manual_seed(7)
+    z = (torch.linspace(2, 6, S, device=DEV)[None, :] + torch.rand(N_RAYS, S, device=DEV, generator=g) * 0.1).contiguous()
+    P = N_RAYS * S
+    ppad = (P + 127) // 128 * 128
+    assert P % 128 != 0
+    st = _lib.stream_ptr(torch.device(DEV))
+
+    raw32 = torch.full((N_RAYS, S, 4), float("nan"), device=DEV)
+    save = {k: torch.full(shape, float("nan"), device=DEV)
+            for k, shape in (("enc", (P, 64)), ("dir", (P, 32)), ("h", (8, P, 256)), ("g", (P, 128)))}
+    _lib.check(lib.snb_field_forward_train(_lib.ptr(img), prec, _lib.ptr(rays), _lib.ptr(z), N_RAYS, S, _lib.ptr(raw32),
+                                           _lib.ptr(save["enc"]), _lib.ptr(save["dir"]), _lib.ptr(save["h"]),
+                                           _lib.ptr(save["g"]), st), "snb_field_forward_train")
+    raw16 = torch.full((N_RAYS, S, 4), float("nan"), device=DEV)
+    act16 = torch.full((lib.snb_act16_bytes(P),), 0xAB, dtype=torch.uint8, device=DEV)   # no cell may keep this
+    _lib.check(lib.snb_field_forward_train16(_lib.ptr(img), prec, _lib.ptr(rays), _lib.ptr(z), N_RAYS, S, _lib.ptr(raw16),
+                                             _lib.ptr(act16), st), "snb_field_forward_train16")
+    torch.cuda.synchronize()
+    assert torch.isfinite(raw32).all()
+    assert_rows_equal(raw16, raw32, f"{precision} raw")
+
+    # act16 sections in order (csrc/act16.cuh): enc, dir, h1..h8, g as fp16 T32 tensors, then the mask words.
+    # Byte offset of the 16-byte cell (p, f8) of a (Ppad, F) tensor: ((p >> 5) * (F >> 3) + f8) * 512 + (p & 31) * 16
+    want = [("enc", save["enc"]), ("dir", save["dir"])] + [(f"h{l + 1}", save["h"][l]) for l in range(8)] + \
+        [("g", save["g"])]
+    off = 0
+    for name, ref in want:
+        F = ref.shape[1]
+        n = ppad * F * 2
+        got = act16[off:off + n].view(torch.int16).reshape(ppad // 32, F // 8, 32, 8).permute(0, 2, 1, 3).reshape(ppad, F)
+        off += n
+        assert_rows_equal(got[:P], ref.clamp(-65504, 65504).half().view(torch.int16), f"{precision} {name}")
+        assert not bool(got[P:].any()), f"{precision} {name}: padded points are not zero"
+    # mask word w of layer l, point p at ((l * 8 + w) * Ppad + p); bit c is [h_{l+1}[p][32 w + c] > 0]
+    mask = act16[off:].view(torch.int32).reshape(8, 8, ppad)
+    bits = (mask[..., None] >> torch.arange(32, device=DEV, dtype=torch.int32)) & 1
+    bits = bits.permute(0, 2, 1, 3).reshape(8, ppad, 256)
+    for l in range(8):
+        assert_rows_equal(bits[l, :P].bool(), save["h"][l] > 0, f"{precision} mask of h{l + 1}")
+    assert not bool(bits[:, P:].any()), f"{precision} mask: padded points are not zero"
