@@ -22,7 +22,7 @@ def get_precision() -> str:
 # one fp16 copy in the MMA-ready tile layout + power-of-two scaled fp16 gradients between layers, backward on
 # tensor cores (half the HBM traffic and memory; parameter gradients within the 1e-3 parity bar).  'fp32':
 # row-major fp32 activations and the fp32-input tensor-core backward (bf16 hi/lo split; the only option of precision
-# 'fp32').  SNB_BWD_SIMT=1 runs that arm's GEMMs on the FFMA kernels instead (A/B reference).
+# 'fp32').
 _train_storage = os.environ.get("SINNERF_B200_TRAIN_STORAGE", "fp16")
 
 

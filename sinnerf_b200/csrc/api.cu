@@ -48,7 +48,6 @@ int launch_sample_pdf(const float*, int64_t, const float*, int64_t, const float*
                       float, float*, cudaStream_t);
 int launch_importance_merge(const float*, const float*, const float*, int64_t, int64_t, int, int, float, float*,
                             float*, cudaStream_t);
-int launch_pack_fp32(const float* const*, int, void*, int, cudaStream_t);
 int field_forward_fp32(const void*, const float*, const float*, int64_t, int, int, float*, cudaStream_t);
 int mlp_forward_fp32(const void*, const float*, int64_t, int64_t, int, float*, cudaStream_t);
 int field_forward_train_fp32(const void*, const float*, const float*, int64_t, int, float*, float*, float*, float*,
@@ -69,7 +68,6 @@ int field_backward16(const float* const*, float* const*, int, const float*, cons
 int adam_step_pack(float* const*, const float* const*, float*, float*, const SnbAdamArgs&, int, int, void*, cudaStream_t);
 // tensor-core modes (field_tc.cu)
 size_t tc_packed_bytes(int precision);
-int launch_pack_tc(const float* const*, int, int, void*, int, cudaStream_t);
 int field_forward_tc(const void*, int, const float*, const float*, int64_t, int, int, float*, cudaStream_t);
 int mlp_forward_tc(const void*, int, const float*, int64_t, int64_t, int, float*, cudaStream_t);
 int field_forward_train_tc(const void*, int, const float*, const float*, int64_t, int, float*, float*, float*, float*,

@@ -14,17 +14,12 @@
 //   layers    : dH_{l-1} = dgrad16(dH_l, W_l) * mask(h_l);  dW_l, db_l = wgrad16(dH_l, h_l)          l = 8 .. 1
 // HBM per point: ~2.5 KB per 256-wide layer (fp32 version: ~5 KB), 4.5 KB of saved activations (8.9 KB).
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 #include "act16.cuh"
 #include "common.cuh"
 
 namespace snb {
 
-// field_bwd.cu
-int launch_fold_weights(const float* Wd, const float* Wf, float* ws, cudaStream_t st);
-int launch_unfold_grads(const float* Wd, const float* Wf, const float* bf, const float* ws, float* dWd, float* dbd,
-                        float* dWf, float* dbf, cudaStream_t st);
 // wgrad16.cu / dgrad16.cu
 int run_wgrad16(const void* dY, int FA, const void* X, int FB, int K, float* dW, int ldw, int col_off, float* db,
                 const float* scale, const void* hg, float* const* dH, const float* scale2, long long n_points_pad,
@@ -34,8 +29,6 @@ int run_dgrad16(const void* dY, const void* dY_lo, int N, const float* W, int ld
                 int st_scale_in, int st_l1, int st_amax_out, int st_scale_out, long long P, cudaStream_t st);
 
 namespace {
-
-constexpr int kFoldW = 0, kFoldDW = kHalf * kWidth, kFoldDB = 2 * kHalf * kWidth;   // offsets into the fold scratch (floats)
 
 // ------------------------------------------------------------------------------------------
 // max |g_raw| when the compositing backward did not provide it (stand-alone use of the C ABI)
@@ -103,7 +96,7 @@ struct Head16Args {
   const float* Wr;           // (3,128)
   int new_activation;
   unsigned char* dS;         // (Ppad,128) fp16 T32, scaled by state[ST_SCALE_DS]
-  unsigned char* dS_lo;      // residual plane (nullable)
+  unsigned char* dS_lo;      // residual plane
   unsigned char* hg;         // (Ppad,8) fp16 T32, scaled by state[ST_SCALE_HG]
   float* dbr; float* dbs;
   float* state;
@@ -176,7 +169,7 @@ __global__ void __launch_bounds__(256) head_bwd16_kernel(Head16Args a) {
         ol[j2] = pack_half2_sat(ds[0] - hv.x, ds[1] - hv.y);
       }
       *reinterpret_cast<uint4*>(a.dS + a16_cell(p, f8, kHalf)) = make_uint4(o[0], o[1], o[2], o[3]);
-      if (a.dS_lo != nullptr) *reinterpret_cast<uint4*>(a.dS_lo + a16_cell(p, f8, kHalf)) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+      *reinterpret_cast<uint4*>(a.dS_lo + a16_cell(p, f8, kHalf)) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
     }
   }
 #pragma unroll
@@ -213,11 +206,8 @@ int field_backward16(const float* const* params, float* const* grads, int new_ac
   auto M = [&](int l) { return mask + (size_t)l * 8 * (size_t)ppad; };   // ReLU mask of h_{l+1}
   // The gradient chain carries its fp16 rounding residual (a second plane) from dS down to dH_4; below that the
   // chain is hi-only: a weight gradient then sees at most 4 chained 11-bit roundings (measured <= 4e-4 rel-L2, parity
-  // bar 1e-3) and the four lowest hops move 1 KB per point instead of 2.  SNB_BWD16_LO = 0: hi-only everywhere
-  // (first-layer gradients ~6e-4), 2: residual planes all the way down (~2.4e-4 flat).
-  static const int lo_mode = getenv("SNB_BWD16_LO") ? atoi(getenv("SNB_BWD16_LO")) : 1;
-  const bool use_lo = lo_mode != 0;
-  const int lo_floor = lo_mode == 2 ? 0 : 4;       // dH_l has a residual plane for l >= lo_floor
+  // bar 1e-3) and the four lowest hops move 1 KB per point instead of 2.  For comparison, a hi-only chain measured
+  // ~6e-4 on the first layer's gradients, residual planes all the way down ~2.4e-4 flat.
   int rc;
   if (cudaMemsetAsync(state, 0, kBwdStateFloats * sizeof(float), st) != cudaSuccess)
     return fail(SNB_ERR_CUDA, "field_backward16: cudaMemsetAsync failed");
@@ -240,7 +230,7 @@ int field_backward16(const float* const* params, float* const* grads, int new_ac
   }
   {
     Head16Args a{reinterpret_cast<const float4*>(g_raw), reinterpret_cast<const float4*>(raw), act + A.g, params[kRgbW],
-                 new_activation, w + B.ds, use_lo ? w + B.ds_lo : nullptr, w + B.hg, grads[kRgbB], grads[kSigmaB], state, P, ppad};
+                 new_activation, w + B.ds, w + B.ds_lo, w + B.hg, grads[kRgbB], grads[kSigmaB], state, P, ppad};
     long long tiles = ppad / 32, blocks = (tiles + 7) / 8;
     if (blocks > sm_count() * 4) blocks = sm_count() * 4;
     head_bwd16_kernel<<<(unsigned)blocks, 256, 0, st>>>(a);
@@ -264,9 +254,9 @@ int field_backward16(const float* const* params, float* const* grads, int new_ac
   // into h8: through W', plus the sigma head's term; ReLU mask of h8
   unsigned char* cur = w + B.dya;
   unsigned char* nxt = w + B.dyb;
-  unsigned char* cur_lo = use_lo ? w + B.dya_lo : nullptr;
-  unsigned char* nxt_lo = use_lo ? w + B.dyb_lo : nullptr;
-  if ((rc = run_dgrad16(w + B.ds, use_lo ? w + B.ds_lo : nullptr, 128, fold + kFoldW, 256, 0, M(7), g_raw + 3, 4, params[kSigmaW], cur,
+  unsigned char* cur_lo = w + B.dya_lo;
+  unsigned char* nxt_lo = w + B.dyb_lo;
+  if ((rc = run_dgrad16(w + B.ds, w + B.ds_lo, 128, fold + kFoldW, 256, 0, M(7), g_raw + 3, 4, params[kSigmaW], cur,
                         cur_lo, state, ST_AMAX_DS, ST_SCALE_DS, ST_L1_FOLD, ST_AMAX_H0 + 7, ST_SCALE_H0 + 7, P, st)))
     return rc;
   for (int l = 7; l >= 1; --l) {
@@ -278,7 +268,7 @@ int field_backward16(const float* const* params, float* const* grads, int new_ac
     } else {
       if ((rc = run_wgrad16(cur, 256, H(l - 1), 256, 256, grads[2 * l], ldw, 0, grads[2 * l + 1], sc, nullptr, nullptr, nullptr, ppad, st))) return rc;
     }
-    const bool lo_in = use_lo && l >= lo_floor, lo_out = use_lo && l - 1 >= lo_floor;
+    const bool lo_in = l >= 4, lo_out = l - 1 >= 4;     // dH_l has a residual plane for l >= 4
     if ((rc = run_dgrad16(cur, lo_in ? cur_lo : nullptr, 256, params[2 * l], ldw, l == 4 ? kXyzCh : 0, M(l - 1), nullptr, 0, nullptr,
                           nxt, lo_out ? nxt_lo : nullptr, state, ST_AMAX_H0 + l, ST_SCALE_H0 + l, ST_L1_L0 + l, ST_AMAX_H0 + l - 1,
                           ST_SCALE_H0 + l - 1, P, st)))

@@ -93,6 +93,31 @@ struct ParamPtrs {
 };
 // enqueues the check kernel: header.dirty = (image was not packed from exactly these values / this mode)
 int launch_params_check(const ParamPtrs& pp, int precision, int new_activation, void* image, cudaStream_t st);
+// the pack kernels (ray_kernels.cu, field_tc.cu); only_if_dirty: return at once unless header.dirty is set
+int launch_pack_fp32(const float* const* params, int new_activation, void* image, int only_if_dirty, cudaStream_t st);
+int launch_pack_tc(const float* const* params, int precision, int new_activation, void* image, int only_if_dirty,
+                   cudaStream_t st);
+
+// One term of the checksum: the 32-bit word of the parameter at flat index `idx` over the 24 concatenated tensors,
+// mixed with its position.  params_check_kernel and adam_step_kernel both sum these and must agree bit for bit:
+// otherwise every pass after an optimiser step sees a stale checksum and re-packs the image.
+__device__ __forceinline__ unsigned long long param_checksum_term(unsigned long long idx, uint32_t word) {
+  unsigned long long x = (idx << 32) ^ (unsigned long long)word ^ 0x9e3779b97f4a7c15ull;
+  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
+  x ^= x >> 27; x *= 0x94d049bb133111ebull;
+  return x ^ (x >> 31);
+}
+
+// ------------------------------------------------------------------ folded bottleneck (field_bwd.cu)
+// Both backward drivers fold the bottleneck into the direction layer: W' = Wd[:, :256] Wf.  Their fold scratch holds
+// W' (128 x 256), then dW' (128 x 256) and db' (128) that the direction layer's wgrad accumulates; offsets in floats.
+constexpr int kFoldW = 0, kFoldDW = kHalf * kWidth, kFoldDB = 2 * kHalf * kWidth;
+static_assert(kFoldDB + kHalf == SNB_BWD_WS_FLOATS, "fold scratch = SNB_BWD_WS_FLOATS floats");
+// fills W' and zeroes dW', db'
+int launch_fold_weights(const float* Wd, const float* Wf, float* ws, cudaStream_t st);
+// accumulates the chain rule from dW', db' back to dWd, dbd, dWf, dbf
+int launch_unfold_grads(const float* Wd, const float* Wf, const float* bf, const float* ws, float* dWd, float* dbd,
+                        float* dWf, float* dbf, cudaStream_t st);
 
 // ------------------------------------------------------------------ fp32 (FFMA) image
 // floats after the header:

@@ -26,12 +26,6 @@ struct AdamPtrs {
   const float* g[SNB_N_PARAM_TENSORS];   // nullable per tensor: no gradient -> tensor skipped (as torch does)
 };
 
-__device__ __forceinline__ unsigned long long mix64_opt(unsigned long long x) {
-  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
-  x ^= x >> 27; x *= 0x94d049bb133111ebull;
-  return x ^ (x >> 31);
-}
-
 __global__ void __launch_bounds__(256) adam_step_kernel(AdamPtrs a, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
                                                         float lr_neg_step, float beta1_w, float beta2, float beta2_w, float eps,
                                                         float weight_decay, float inv_bc2_sqrt, int precision, int new_activation,
@@ -57,7 +51,7 @@ __global__ void __launch_bounds__(256) adam_step_kernel(AdamPtrs a, float* __res
         exp_avg_sq[base + e] = v;
         p[e] = w;
       }
-      h += mix64_opt(((base + e) << 32) ^ (unsigned long long)__float_as_uint(w) ^ 0x9e3779b97f4a7c15ull);
+      h += param_checksum_term(base + e, __float_as_uint(w));
     }
     base += n;
   }
@@ -82,9 +76,6 @@ __global__ void __launch_bounds__(256) adam_step_kernel(AdamPtrs a, float* __res
     }
   }
 }
-
-int launch_pack_fp32(const float* const*, int, void*, int, cudaStream_t);
-int launch_pack_tc(const float* const*, int, int, void*, int, cudaStream_t);
 
 int adam_step_pack(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
                    const SnbAdamArgs& o, int precision, int new_activation, void* packed, cudaStream_t st) {

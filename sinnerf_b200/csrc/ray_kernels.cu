@@ -847,11 +847,6 @@ constexpr int kCheckBlocks = 146, kCheckThreads = 1024;
 static_assert(kCheckBlocks * kCheckThreads * 4 >= SNB_PARAM_FLOATS &&
                   (kCheckBlocks - 1) * kCheckThreads * 4 < SNB_PARAM_FLOATS,
               "params_check_kernel: smallest one-pass grid");
-__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
-  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
-  x ^= x >> 27; x *= 0x94d049bb133111ebull;
-  return x ^ (x >> 31);
-}
 __global__ void __launch_bounds__(kCheckThreads) params_check_kernel(ParamPtrs pp, int precision, int new_activation,
                                                                      PackedHeader* hdr) {
   // flat index g over the concatenated tensors (the position the checksum mixes in): every thread owns g = gid + k T,
@@ -883,13 +878,12 @@ __global__ void __launch_bounds__(kCheckThreads) params_check_kernel(ParamPtrs p
   unsigned long long h = 0;
 #pragma unroll
   for (int k = 0; k < 4; ++k)
-    if (gi[k] >= 0) h += mix64(((unsigned long long)gi[k] << 32) ^ (unsigned long long)w[k] ^ 0x9e3779b97f4a7c15ull);
+    if (gi[k] >= 0) h += param_checksum_term(gi[k], w[k]);
   for (int g = blockIdx.x * blockDim.x + threadIdx.x + 4 * stride; g < total; g += stride) {   // (grids smaller than total / 4)
     int t = 0;
     for (int step = 16; step > 0; step >>= 1)
       if (t + step < SNB_N_PARAM_TENSORS && s_off[t + step] <= g) t += step;
-    h += mix64(((unsigned long long)g << 32) ^ (unsigned long long)__ldg(reinterpret_cast<const unsigned int*>(pp.p[t]) + (g - s_off[t])) ^
-               0x9e3779b97f4a7c15ull);
+    h += param_checksum_term(g, __ldg(reinterpret_cast<const unsigned int*>(pp.p[t]) + (g - s_off[t])));
   }
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) h += __shfl_xor_sync(kFull, h, off);
@@ -967,12 +961,11 @@ static int grid_for(long long work_items, int per_block, int cap_blocks) {
   if (b < 1) b = 1;
   return (int)(b < cap_blocks ? b : cap_blocks);
 }
-static int device_sms() { return sm_count(); }
 
 int launch_sample_coarse(const float* rays, const float* z_steps, const float* perturb_u, float perturb,
                          int use_disp, int64_t n_rays, int S, float* z, cudaStream_t st) {
   if (n_rays == 0) return SNB_OK;
-  const int grid = grid_for(n_rays * S, 256, device_sms() * 8);
+  const int grid = grid_for(n_rays * S, 256, sm_count() * 8);
   sample_coarse_kernel<<<grid, 256, 0, st>>>(rays, z_steps, perturb_u, perturb, use_disp, n_rays, S, z);
   return check_launch("sample_coarse_kernel");
 }
@@ -986,14 +979,14 @@ int launch_generate_rays(const float* c2w_host, float fx, float fy, float cx, fl
   a.row0 = row0; a.col0 = col0; a.rows = rows; a.cols = cols; a.stride = stride; a.rays = rays;
   const long long n = (long long)rows * cols;
   if (n == 0) return SNB_OK;
-  generate_rays_kernel<<<grid_for(n, 256, device_sms() * 8), 256, 0, st>>>(a);
+  generate_rays_kernel<<<grid_for(n, 256, sm_count() * 8), 256, 0, st>>>(a);
   return check_launch("generate_rays_kernel");
 }
 
 int launch_embed(const float* x, int64_t n, int C, int L, float* out, cudaStream_t st) {
   if (n == 0) return SNB_OK;
   if (C == 3 && (L == SNB_XYZ_FREQS || L == SNB_DIR_FREQS) && (reinterpret_cast<uintptr_t>(out) & 15) == 0) {
-    const int grid3 = grid_for(n, kEmbedRows, device_sms() * 6);
+    const int grid3 = grid_for(n, kEmbedRows, sm_count() * 6);
     if (L == SNB_XYZ_FREQS) embed3_kernel<SNB_XYZ_FREQS><<<grid3, 256, 0, st>>>(x, n, out);
     else embed3_kernel<SNB_DIR_FREQS><<<grid3, 256, 0, st>>>(x, n, out);
     return check_launch("embed3_kernel");
@@ -1003,7 +996,7 @@ int launch_embed(const float* x, int64_t n, int C, int L, float* out, cudaStream
   static SmemOptIn optin;
   if (smem > 48 * 1024)
     if (int rc = ensure_smem(embed_kernel, optin, (int)smem, "embed")) return rc;
-  const int grid = grid_for(n, kEmbedRows, device_sms() * 4);
+  const int grid = grid_for(n, kEmbedRows, sm_count() * 4);
   embed_kernel<<<grid, 256, smem, st>>>(x, n, C, L, out);
   return check_launch("embed_kernel");
 }
@@ -1039,11 +1032,10 @@ int launch_composite(const float* raw, int raw_channels, const float* z, const f
                                         ? SNB_OK : fail(SNB_ERR_CUDA, "cudaMemsetAsync(loss)");
     return SNB_OK;
   }
-  static const bool warp_per_ray = getenv("SNB_COMPOSITE_WARP_PER_RAY") != nullptr;   // A/B timing of the two mappings
-  if (composite_quad_ok(S, raw, z, noise, w) && !warp_per_ray) {
+  if (composite_quad_ok(S, raw, z, noise, w)) {
     // four samples per thread: the ray's S/4 threads in a lane group of L = 8 / 16 / 32, 32 / L rays per warp pass
     const int L = S <= 32 ? 8 : (S <= 64 ? 16 : 32);
-    int grid = grid_for(n_rays, 8 * (32 / L), device_sms() * 8);
+    int grid = grid_for(n_rays, 8 * (32 / L), sm_count() * 8);
     if (loss_out != nullptr && grid > (SNB_LOSS_WS_FLOATS - 4) / 2) grid = (SNB_LOSS_WS_FLOATS - 4) / 2;
     const LossSpec ls = make_loss_spec(loss);
     if (L == 8) composite_fwd4_kernel<8><<<grid, 256, 0, st>>>(raw, raw_channels, z, rays, noise, noise_std, white_back, n_rays, S, rgb, depth, w, ls, loss_out, loss_ws, ps);
@@ -1051,7 +1043,7 @@ int launch_composite(const float* raw, int raw_channels, const float* z, const f
     else composite_fwd4_kernel<32><<<grid, 256, 0, st>>>(raw, raw_channels, z, rays, noise, noise_std, white_back, n_rays, S, rgb, depth, w, ls, loss_out, loss_ws, ps);
     return check_launch("composite_fwd4_kernel");
   }
-  int grid = grid_for(n_rays, 8, device_sms() * 8);
+  int grid = grid_for(n_rays, 8, sm_count() * 8);
   if (loss_out != nullptr && grid > (SNB_LOSS_WS_FLOATS - 4) / 2) grid = (SNB_LOSS_WS_FLOATS - 4) / 2;
   composite_fwd_kernel<<<grid, 256, 0, st>>>(raw, raw_channels, z, rays, noise, noise_std, white_back, n_rays,
                                              S, rgb, depth, w, make_loss_spec(loss), loss_out, loss_ws, ps);
@@ -1063,10 +1055,9 @@ int launch_composite_bwd(const float* raw, const float* z, const float* rays, co
                           int S, float* g_raw, const SnbLossSpec* loss, const float* out_rgb, const float* out_depth,
                           const float* g_loss, float* g_amax, cudaStream_t st) {
   if (n_rays == 0) return SNB_OK;
-  static const bool warp_per_ray = getenv("SNB_COMPOSITE_WARP_PER_RAY") != nullptr;
-  if (composite_quad_ok(S, raw, z, noise, g_w) && (reinterpret_cast<uintptr_t>(g_raw) & 15) == 0 && !warp_per_ray) {
+  if (composite_quad_ok(S, raw, z, noise, g_w) && (reinterpret_cast<uintptr_t>(g_raw) & 15) == 0) {
     const int L = S <= 32 ? 8 : (S <= 64 ? 16 : 32);
-    const int grid = grid_for(n_rays, 8 * (32 / L), device_sms() * 6);
+    const int grid = grid_for(n_rays, 8 * (32 / L), sm_count() * 6);
     const LossSpec ls = make_loss_spec(loss);
     unsigned int* am = reinterpret_cast<unsigned int*>(g_amax);
     if (L == 8) composite_bwd4_kernel<8><<<grid, 256, 0, st>>>(raw, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w, n_rays, S, g_raw, ls, out_rgb, out_depth, g_loss, am);
@@ -1079,7 +1070,7 @@ int launch_composite_bwd(const float* raw, const float* z, const float* rays, co
   static SmemOptIn optin;
   if (smem > 48 * 1024)
     if (int rc = ensure_smem(composite_bwd_kernel, optin, (int)smem, "composite_bwd")) return rc;
-  const int grid = grid_for(n_rays, 8, device_sms() * 8);
+  const int grid = grid_for(n_rays, 8, sm_count() * 8);
   composite_bwd_kernel<<<grid, 256, smem, st>>>(raw, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w,
                                                 n_rays, S, g_raw, make_loss_spec(loss), out_rgb, out_depth, g_loss,
                                                 reinterpret_cast<unsigned int*>(g_amax));
@@ -1092,7 +1083,7 @@ int launch_sample_pdf(const float* bins, int64_t bins_stride, const float* weigh
   if (n_rays == 0) return SNB_OK;
   const size_t smem = (size_t)4 * (M + 1) * sizeof(float);
   if (smem > 48 * 1024) return fail(SNB_ERR_UNSUPPORTED, "snb_sample_pdf: too many bins (%d)", M);
-  const int grid = grid_for(n_rays, 4, device_sms() * 16);
+  const int grid = grid_for(n_rays, 4, sm_count() * 16);
   sample_pdf_kernel<<<grid, 128, smem, st>>>(bins, bins_stride, weights, w_stride, u, u_stride, n_rays, M, Ni,
                                              eps, out);
   return check_launch("sample_pdf_kernel");
@@ -1105,7 +1096,7 @@ int launch_importance_merge(const float* z_coarse, const float* w_coarse, const 
   if (Ni > 256) return fail(SNB_ERR_UNSUPPORTED, "snb_importance_merge: N_importance > 256 (%d)", Ni);
   const size_t smem = (size_t)4 * ((S - 1) + (S + Ni)) * sizeof(float);
   if (smem > 48 * 1024) return fail(SNB_ERR_UNSUPPORTED, "snb_importance_merge: S+Ni too large");
-  const int grid = grid_for(n_rays, 4, device_sms() * 16);
+  const int grid = grid_for(n_rays, 4, sm_count() * 16);
   importance_merge_kernel<<<grid, 128, smem, st>>>(z_coarse, w_coarse, u, u_stride, n_rays, S, Ni, eps, z_fine,
                                                    z_new);
   return check_launch("importance_merge_kernel");
@@ -1114,7 +1105,7 @@ int launch_importance_merge(const float* z_coarse, const float* w_coarse, const 
 int launch_pack_fp32(const float* const* params, int new_activation, void* image, int only_if_dirty, cudaStream_t st) {
   ParamPtrs pp;
   for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) pp.p[i] = params[i];
-  pack_fp32_kernel<<<device_sms() * 2, 256, 0, st>>>(pp, new_activation, reinterpret_cast<unsigned char*>(image), only_if_dirty);
+  pack_fp32_kernel<<<sm_count() * 2, 256, 0, st>>>(pp, new_activation, reinterpret_cast<unsigned char*>(image), only_if_dirty);
   return check_launch("pack_fp32_kernel");
 }
 
