@@ -255,6 +255,34 @@ typedef struct SnbAdamArgs {
 int snb_adam_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
                   const SnbAdamArgs* args, int precision, int new_activation, void* packed, void* stream);
 
+/* The reference's other get_optimizer choices (utils/__init__.py:15-27), same launch shape, checksum stamp and
+ * re-pack as snb_adam_step:
+ *   SNB_OPTIM_SGD     torch.optim.SGD(lr, momentum, weight_decay), dampening 0, no Nesterov.  exp_avg = the
+ *                     momentum buffer; exp_avg_sq / slow_buffer unused (may be NULL).
+ *   SNB_OPTIM_RADAM   utils/optimizers.py:7-106 (degenerated_to_sgd = True); slow_buffer unused (may be NULL).
+ *   SNB_OPTIM_RANGER  utils/optimizers.py:292-439: RAdam moments + lookahead every k-th step into slow_buffer.
+ * step[i] is tensor i's update count INCLUDING this one (the reference's state['step'] after its increment; for
+ * SGD: the momentum-buffer update count, 1 = the buffer is a copy of the gradient).  Each tensor is stepped by its
+ * own count, so one that had no gradient on earlier steps gets the same scalars the reference gives it; step[i] is
+ * ignored where grads[i] is NULL.  RAdam / Ranger: N_sma and step_size are formed per tensor on the host in double,
+ * in the reference's expression order.  Buffers are SNB_PARAM_FLOATS floats, like snb_adam_step's. */
+#define SNB_OPTIM_SGD 0
+#define SNB_OPTIM_RADAM 1
+#define SNB_OPTIM_RANGER 2
+typedef struct SnbOptimArgs {
+  int rule;                          /* SNB_OPTIM_*                                                      */
+  double lr, weight_decay;
+  double momentum;                   /* SGD                                                              */
+  double beta1, beta2, eps;          /* RAdam / Ranger                                                   */
+  double n_sma_threshold;            /* Ranger: adaptive step iff N_sma > threshold (RAdam: N_sma >= 5)   */
+  double alpha;                      /* Ranger: slow += alpha * (p - slow) ...                           */
+  int k;                             /* ... every k-th step of the tensor, then p = slow                 */
+  int step[SNB_N_PARAM_TENSORS];
+} SnbOptimArgs;
+int snb_optim_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
+                   float* slow_buffer, const SnbOptimArgs* args, int precision, int new_activation, void* packed,
+                   void* stream);
+
 /* ---- whole path -------------------------------------------------------------------- */
 typedef struct SnbRenderArgs {
   const float* rays;        /* (N,8)                                                    */

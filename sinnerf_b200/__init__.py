@@ -13,7 +13,7 @@ def __getattr__(name):
     if name in ("NeRF", "Embedding"):
         from . import nerf
         return getattr(nerf, name)
-    if name in ("FusedAdam", "get_optimizer"):
+    if name in ("FusedAdam", "FusedSGD", "FusedRAdam", "FusedRanger", "get_optimizer"):
         from . import optim
         return getattr(optim, name)
     raise AttributeError(name)

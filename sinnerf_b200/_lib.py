@@ -49,6 +49,15 @@ class SnbAdamArgs(C.Structure):
                 ("weight_decay", C.c_double), ("step", C.c_int)]
 
 
+OPTIM_SGD, OPTIM_RADAM, OPTIM_RANGER = 0, 1, 2   # SNB_OPTIM_*
+
+
+class SnbOptimArgs(C.Structure):
+    _fields_ = [("rule", C.c_int), ("lr", C.c_double), ("weight_decay", C.c_double), ("momentum", C.c_double),
+                ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double), ("n_sma_threshold", C.c_double),
+                ("alpha", C.c_double), ("k", C.c_int), ("step", C.c_int * 24)]
+
+
 LOSS_WS_FLOATS = 4096   # SNB_LOSS_WS_FLOATS
 PARAM_FLOATS = 595844   # SNB_PARAM_FLOATS
 
@@ -88,6 +97,8 @@ SIGNATURES = {
                                        c_f, c_f, c_f]),
     "snb_adam_step": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, C.POINTER(SnbAdamArgs),
                                 C.c_int, C.c_int, c_f, c_f]),
+    "snb_optim_step": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, c_f, C.POINTER(SnbOptimArgs),
+                                 C.c_int, C.c_int, c_f, c_f]),
     "snb_field_backward": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, c_f, c_f, c_f, c_f, c_f,
                                      c_f, C.c_int64, c_f, c_f, c_f, c_f, c_f, c_f]),
 }

@@ -66,6 +66,8 @@ size_t bwd16_workspace_bytes(long long);
 int field_backward16(const float* const*, float* const*, int, const float*, const float*, const void*, long long, void*,
                      const float*, cudaStream_t);
 int adam_step_pack(float* const*, const float* const*, float*, float*, const SnbAdamArgs&, int, int, void*, cudaStream_t);
+int optim_step_pack(float* const*, const float* const*, float*, float*, float*, const SnbOptimArgs&, int, int, void*,
+                    cudaStream_t);
 // tensor-core modes (field_tc.cu)
 size_t tc_packed_bytes(int precision);
 int field_forward_tc(const void*, int, const float*, const float*, int64_t, int, int, float*, cudaStream_t);
@@ -367,6 +369,32 @@ int snb_adam_step(float* const* params, const float* const* grads, float* exp_av
   static_assert(SNB_PARAM_FLOATS == 593408 + 2436, "parameter count");
   return adam_step_pack(params, grads, exp_avg, exp_avg_sq, *args, precision, new_activation, packed,
                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_optim_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
+                   float* slow_buffer, const SnbOptimArgs* args, int precision, int new_activation, void* packed,
+                   void* stream) {
+  SNB_REQUIRE(params && grads && args, "snb_optim_step: null pointer");
+  const int rule = args->rule;
+  SNB_REQUIRE(rule == SNB_OPTIM_SGD || rule == SNB_OPTIM_RADAM || rule == SNB_OPTIM_RANGER,
+              "snb_optim_step: unknown rule %d", rule);
+  SNB_REQUIRE(exp_avg != nullptr && (rule == SNB_OPTIM_SGD || exp_avg_sq != nullptr) &&
+                  (rule != SNB_OPTIM_RANGER || slow_buffer != nullptr),
+              "snb_optim_step: null state buffer");
+  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) {
+    SNB_REQUIRE(params[i] != nullptr, "snb_optim_step: parameter tensor %d is null", i);
+    SNB_REQUIRE(grads[i] == nullptr || args->step[i] >= 1 || (rule == SNB_OPTIM_SGD && args->momentum == 0.),
+                "snb_optim_step: step of tensor %d counts from 1 (got %d)", i, args->step[i]);
+  }
+  SNB_REQUIRE(args->lr >= 0. && args->weight_decay >= 0. && args->momentum >= 0. && args->eps >= 0. &&
+                  args->beta1 >= 0. && args->beta1 < 1. && args->beta2 >= 0. && args->beta2 < 1. &&
+                  args->alpha >= 0. && args->alpha <= 1. && args->k >= 1,
+              "snb_optim_step: invalid hyper-parameters");
+  SNB_REQUIRE(packed == nullptr || aligned16(packed), "snb_optim_step: packed image must be 16-byte aligned");
+  if (packed != nullptr)
+    if (int rc = check_precision(precision)) return rc;
+  return optim_step_pack(params, grads, exp_avg, exp_avg_sq, slow_buffer, *args, precision, new_activation, packed,
+                         reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_render_forward(const SnbRenderArgs* a, void* stream) {

@@ -1,5 +1,5 @@
-// optim.cu -- fused Adam step over the 24 parameter tensors of one NeRF + refresh of its packed image
-// (SURVEY.md 8f-4).  Reference: get_optimizer -> torch.optim.Adam(lr, eps=1e-8, weight_decay)
+// optim.cu -- fused optimiser step (Adam; SGD / RAdam / Ranger further down) over the 24 parameter tensors of one
+// NeRF + refresh of its packed image (SURVEY.md 8f-4).  Reference: get_optimizer -> torch.optim.Adam(lr, eps=1e-8, weight_decay)
 // (utils/__init__.py:19-21), stepped once per training iteration by Lightning (train.py:51-52 under DDP,
 // i.e. after the gradient all-reduce).
 //
@@ -25,6 +25,30 @@ struct AdamPtrs {
   float* p[SNB_N_PARAM_TENSORS];
   const float* g[SNB_N_PARAM_TENSORS];   // nullable per tensor: no gradient -> tensor skipped (as torch does)
 };
+
+// Block-reduces each thread's checksum sum and, in the last block to finish, stamps the image header with the
+// checksum of the NEW values (the same sum params_check_kernel computes).
+__device__ __forceinline__ void stamp_checksum(unsigned long long h, PackedHeader* hdr) {
+  if (hdr == nullptr) return;
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) h += __shfl_xor_sync(0xffffffffu, h, off);
+  __shared__ unsigned long long part[8];
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = h;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long b = 0;
+    for (int i = 0; i < 8; ++i) b += part[i];
+    atomicAdd(&hdr->partial, b);
+    __threadfence();
+    if (atomicAdd(&hdr->blocks_done, 1u) == gridDim.x - 1) {
+      __threadfence();
+      hdr->checksum = atomicAdd(&hdr->partial, 0ull);
+      hdr->dirty = 1;                  // the pack kernels that follow run unconditionally; keep the flag truthful
+      hdr->partial = 0ull;
+      hdr->blocks_done = 0u;
+    }
+  }
+}
 
 __global__ void __launch_bounds__(256) adam_step_kernel(AdamPtrs a, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
                                                         float lr_neg_step, float beta1_w, float beta2, float beta2_w, float eps,
@@ -55,26 +79,16 @@ __global__ void __launch_bounds__(256) adam_step_kernel(AdamPtrs a, float* __res
     }
     base += n;
   }
-  if (hdr == nullptr) return;
-  // stamp the image header with the checksum of the NEW values (same sum params_check_kernel computes)
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) h += __shfl_xor_sync(0xffffffffu, h, off);
-  __shared__ unsigned long long part[8];
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = h;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned long long b = 0;
-    for (int i = 0; i < 8; ++i) b += part[i];
-    atomicAdd(&hdr->partial, b);
-    __threadfence();
-    if (atomicAdd(&hdr->blocks_done, 1u) == gridDim.x - 1) {
-      __threadfence();
-      hdr->checksum = atomicAdd(&hdr->partial, 0ull);
-      hdr->dirty = 1;                  // the pack kernels that follow run unconditionally; keep the flag truthful
-      hdr->partial = 0ull;
-      hdr->blocks_done = 0u;
-    }
-  }
+  stamp_checksum(h, hdr);
+}
+
+// The image the forward streams, re-packed on the step's stream from the updated parameters (packed == NULL: none).
+static int repack(float* const* params, int precision, int new_activation, void* packed, cudaStream_t st) {
+  if (packed == nullptr) return SNB_OK;
+  const float* cp[SNB_N_PARAM_TENSORS];
+  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) cp[i] = params[i];
+  if (precision == SNB_PREC_FP32) return launch_pack_fp32(cp, new_activation ? 1 : 0, packed, 0, st);
+  return launch_pack_tc(cp, precision, new_activation ? 1 : 0, packed, 0, st);
 }
 
 int adam_step_pack(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
@@ -91,11 +105,136 @@ int adam_step_pack(float* const* params, const float* const* grads, float* exp_a
                                                   (float)o.eps, (float)o.weight_decay, inv_bc2_sqrt, precision, new_activation,
                                                   reinterpret_cast<PackedHeader*>(packed));
   if (int rc = check_launch("adam_step_kernel")) return rc;
-  if (packed == nullptr) return SNB_OK;
-  const float* cp[SNB_N_PARAM_TENSORS];
-  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) cp[i] = params[i];
-  if (precision == SNB_PREC_FP32) return launch_pack_fp32(cp, new_activation ? 1 : 0, packed, 0, st);
-  return launch_pack_tc(cp, precision, new_activation ? 1 : 0, packed, 0, st);
+  return repack(params, precision, new_activation, packed, st);
+}
+
+// ---------------------------------------------------------------- SGD / RAdam / Ranger (snb_optim_step)
+// Each line is one ATen elementwise kernel of the reference's step, rounded to fp32 as that kernel rounds it
+// (ATen's CUDA add / addcmul / addcdiv contract `a + alpha * b` into one FMA; mul, sqrt, div round on their own):
+//   SGD (torch/optim/sgd.py _multi_tensor_sgd, dampening 0, no Nesterov):
+//     g = g + wd * p                 (_foreach_add, alpha)
+//     b = g (first step)  |  b = b * momentum;  b = b + g         (_foreach_mul_, _foreach_add_)
+//     p = p + (-lr) * b              (_foreach_add_, alpha)
+//   RAdam / Ranger (utils/optimizers.py:65-66,90-104 / :393-425):
+//     v = v * beta2;  v = v + (1 - beta2) * g * g                 (mul_, addcmul_)
+//     m = m * beta1;  m = m + (1 - beta1) * g                     (mul_, add_)
+//     p = p + (-wd * lr) * p                                      (add_, when wd != 0)
+//     p = p + (-step_size * lr) * (m / (sqrt(v) + eps))  if N_sma passes the threshold,   (sqrt, add_, addcdiv_)
+//     p = p + (-step_size * lr) * m                       otherwise                        (add_)
+//   Ranger, every k-th step of the tensor (:431-437): slow = slow + alpha * (p - slow);  p = slow    (sub, add_, copy_)
+//   with slow = p (before the update) on the tensor's first step.
+enum : unsigned { kFirst = 1u, kAdaptive = 2u, kSync = 4u };
+
+struct RuleScalars {
+  float lr_neg;         // SGD: -lr
+  float decay;          // SGD: weight_decay;  RAdam / Ranger: -weight_decay * lr
+  float momentum;       // SGD
+  float beta1, beta1_w, beta2, beta2_w, eps, alpha;
+  float step_lr[SNB_N_PARAM_TENSORS];           // RAdam / Ranger: -step_size * lr at the tensor's own step
+  unsigned char flags[SNB_N_PARAM_TENSORS];     // kFirst | kAdaptive | kSync
+};
+
+template <int RULE>
+__global__ void __launch_bounds__(256) optim_step_kernel(AdamPtrs a, float* __restrict__ exp_avg,
+                                                         float* __restrict__ exp_avg_sq, float* __restrict__ slow_buffer,
+                                                         RuleScalars s, PackedHeader* hdr) {
+  unsigned long long h = 0;
+  unsigned long long base = 0;
+  for (int t = 0; t < SNB_N_PARAM_TENSORS; ++t) {
+    const int n = param_numel(t);
+    float* p = a.p[t];
+    const float* g = a.g[t];
+    const unsigned f = s.flags[t];
+    const float step_lr = s.step_lr[t];
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
+      float w = p[e];
+      if (g != nullptr) {
+        float gr = g[e];
+        const unsigned long long i = base + e;
+        if (RULE == SNB_OPTIM_SGD) {
+          if (s.decay != 0.f) gr = fmaf(s.decay, w, gr);
+          if (s.momentum != 0.f) {
+            if (!(f & kFirst)) gr = __fadd_rn(__fmul_rn(exp_avg[i], s.momentum), gr);
+            exp_avg[i] = gr;
+          }
+          w = fmaf(s.lr_neg, gr, w);
+        } else {
+          float v = __fmul_rn(exp_avg_sq[i], s.beta2);
+          v = fmaf(__fmul_rn(s.beta2_w, gr), gr, v);
+          float m = __fmul_rn(exp_avg[i], s.beta1);
+          m = fmaf(s.beta1_w, gr, m);
+          exp_avg[i] = m;
+          exp_avg_sq[i] = v;
+          float slow = 0.f;
+          if (RULE == SNB_OPTIM_RANGER) slow = (f & kFirst) ? w : slow_buffer[i];
+          if (s.decay != 0.f) w = fmaf(s.decay, w, w);
+          if (f & kAdaptive)
+            w = fmaf(step_lr, __fdiv_rn(m, __fadd_rn(__fsqrt_rn(v), s.eps)), w);
+          else
+            w = fmaf(step_lr, m, w);
+          if (RULE == SNB_OPTIM_RANGER) {
+            if (f & kSync) {
+              slow = fmaf(s.alpha, __fsub_rn(w, slow), slow);
+              w = slow;
+            }
+            if (f & (kFirst | kSync)) slow_buffer[i] = slow;
+          }
+        }
+        p[e] = w;
+      }
+      h += param_checksum_term(base + e, __float_as_uint(w));
+    }
+    base += n;
+  }
+  stamp_checksum(h, hdr);
+}
+
+int optim_step_pack(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
+                    float* slow_buffer, const SnbOptimArgs& o, int precision, int new_activation, void* packed,
+                    cudaStream_t st) {
+  AdamPtrs a;
+  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) { a.p[i] = params[i]; a.g[i] = grads[i]; }
+  RuleScalars s = {};
+  if (o.rule == SNB_OPTIM_SGD) {
+    s.lr_neg = (float)(-o.lr);
+    s.decay = (float)o.weight_decay;
+    s.momentum = (float)o.momentum;
+    for (int t = 0; t < SNB_N_PARAM_TENSORS; ++t) s.flags[t] = o.step[t] == 1 ? kFirst : 0u;
+  } else {
+    s.beta1 = (float)o.beta1;
+    s.beta1_w = (float)(1.0 - o.beta1);
+    s.beta2 = (float)o.beta2;
+    s.beta2_w = (float)(1.0 - o.beta2);
+    s.eps = (float)o.eps;
+    s.alpha = (float)o.alpha;
+    s.decay = (float)(-o.weight_decay * o.lr);
+    for (int t = 0; t < SNB_N_PARAM_TENSORS; ++t) {
+      if (grads[t] == nullptr) continue;
+      // utils/optimizers.py:68-86 / :397-411 in python doubles, the reference's expression order
+      const int step = o.step[t];
+      const double beta2_t = pow(o.beta2, (double)step);
+      const double n_sma_max = 2 / (1 - o.beta2) - 1;
+      const double n_sma = n_sma_max - 2 * step * beta2_t / (1 - beta2_t);
+      const bool adaptive = o.rule == SNB_OPTIM_RADAM ? n_sma >= 5 : n_sma > o.n_sma_threshold;
+      const double step_size =
+          adaptive ? sqrt((1 - beta2_t) * (n_sma - 4) / (n_sma_max - 4) * (n_sma - 2) / n_sma * n_sma_max /
+                          (n_sma_max - 2)) / (1 - pow(o.beta1, (double)step))
+                   : 1.0 / (1 - pow(o.beta1, (double)step));
+      s.step_lr[t] = (float)(-step_size * o.lr);
+      s.flags[t] = (adaptive ? kAdaptive : 0u) | (step == 1 ? kFirst : 0u) |
+                   (o.rule == SNB_OPTIM_RANGER && step % o.k == 0 ? kSync : 0u);
+    }
+  }
+  PackedHeader* hdr = reinterpret_cast<PackedHeader*>(packed);
+  const int grid = sm_count() * 2;
+  if (o.rule == SNB_OPTIM_SGD)
+    optim_step_kernel<SNB_OPTIM_SGD><<<grid, 256, 0, st>>>(a, exp_avg, exp_avg_sq, slow_buffer, s, hdr);
+  else if (o.rule == SNB_OPTIM_RADAM)
+    optim_step_kernel<SNB_OPTIM_RADAM><<<grid, 256, 0, st>>>(a, exp_avg, exp_avg_sq, slow_buffer, s, hdr);
+  else
+    optim_step_kernel<SNB_OPTIM_RANGER><<<grid, 256, 0, st>>>(a, exp_avg, exp_avg_sq, slow_buffer, s, hdr);
+  if (int rc = check_launch("optim_step_kernel")) return rc;
+  return repack(params, precision, new_activation, packed, st);
 }
 
 }  // namespace snb

@@ -164,7 +164,7 @@ class NeRF(nn.Module):
 
     def packed_image_buffer(self, prec: int) -> torch.Tensor:
         """The (precision, device) image buffer, allocated zero-filled on first use; its CONTENT is brought up
-        to date by packed_weights() / FusedAdam.step()."""
+        to date by packed_weights() / the fused optimisers' step()."""
         self._check_shape()
         ps = self._param_list()
         dev = ps[0].device
