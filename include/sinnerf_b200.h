@@ -238,6 +238,39 @@ int snb_field_backward(const float* const* params, float* const* grads, int new_
                        const float* save_h, const float* save_g, int64_t n_points, float* ws_a, float* ws_b,
                        float* ws_s, float* ws_w, uint32_t* ws_m, void* stream);
 
+/* ---- sigma-only training passes ----------------------------------------------------------------------
+ * The field pass of render_rays(test_time=True)'s coarse model (models/rendering.py:287-292, weights_only=True)
+ * and of eval_points (models/rendering.py:64-123) under autograd: layers 1-8 and the sigma head, no direction
+ * layer, no rgb head (models/nerf.py:105-136 with sigma_only=True).
+ *
+ * snb_field_forward_train_sigma / snb_field_forward_train16_sigma: the sigma-only field pass keeping what the
+ * sigma-only backward reads; sigma (N,S) = (P,).  The fp32-storage form keeps save_enc (P,64) and
+ * save_h (8,P,256) as snb_field_forward_train does; the 16-bit form fills the enc, h1..h8 and ReLU-mask
+ * sections of an snb_act16_bytes(P) buffer (the direction sections are left unwritten). */
+int snb_field_forward_train_sigma(const void* packed, int precision, const float* rays, const float* z_vals,
+                                  int64_t n_rays, int n_samples, float* sigma, float* save_enc, float* save_h,
+                                  void* stream);
+int snb_field_forward_train16_sigma(const void* packed, int precision, const float* rays, const float* z_vals,
+                                    int64_t n_rays, int n_samples, float* sigma, void* act16, void* stream);
+/* Backward of models/rendering.py:215-238 with weights_only (closed form, SURVEY.md 8a-7 with g_rgb = g_depth = 0):
+ * g_weights (N,S) -> g_sigma (N,S).  sigma: what the sigma-only forward wrote.  g_amax (nullable): as in
+ * snb_composite_backward_loss, raised to the bit pattern of max |g_sigma| (zero it first). */
+int snb_composite_backward_weights(const float* sigma, const float* z_vals, const float* rays, const float* noise,
+                                   float noise_std, const float* g_weights, int64_t n_rays, int n_samples,
+                                   float* g_sigma, float* g_amax, void* stream);
+/* Backward of a sigma-only field pass (autograd through models/nerf.py:105-136): g_sigma (P,) -> gradients of
+ * xyz_encoding_1..8 and sigma (grads 0..15, 20, 21, ACCUMULATED into).  The entries for xyz_encoding_final,
+ * dir_encoding and rgb (16..19, 22, 23) are neither read nor written and may be NULL in both arrays.
+ * fp32 storage: scratch ws_a, ws_b (P,256) fp32 and ws_m (P,8) 32-bit words, all 16-byte aligned.
+ * 16-bit storage: workspace of snb_bwd16_workspace_bytes(P) bytes; g_amax as snb_composite_backward_weights
+ * leaves it, or NULL (the library then reduces g_sigma itself). */
+int snb_field_backward_sigma(const float* const* params, float* const* grads, const float* g_sigma,
+                             const float* save_enc, const float* save_h, int64_t n_points, float* ws_a, float* ws_b,
+                             uint32_t* ws_m, void* stream);
+int snb_field_backward16_sigma(const float* const* params, float* const* grads, const float* g_sigma,
+                               const void* act16, int64_t n_points, void* workspace, const float* g_amax,
+                               void* stream);
+
 /* ---- optimiser step (SURVEY.md 8f-4) --------------------------------------------------------------
  * torch.optim.Adam as the reference configures it (utils/__init__.py:19-21: lr, eps = 1e-8, weight_decay;
  * betas default (0.9, 0.999), amsgrad off), fused over the 24 parameter tensors of one NeRF, followed on the

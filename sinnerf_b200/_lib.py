@@ -101,6 +101,13 @@ SIGNATURES = {
                                  C.c_int, C.c_int, c_f, c_f]),
     "snb_field_backward": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, c_f, c_f, c_f, c_f, c_f,
                                      c_f, C.c_int64, c_f, c_f, c_f, c_f, c_f, c_f]),
+    "snb_field_forward_train_sigma": (C.c_int, [c_f, C.c_int, c_f, c_f, C.c_int64, C.c_int, c_f, c_f, c_f, c_f]),
+    "snb_field_forward_train16_sigma": (C.c_int, [c_f, C.c_int, c_f, c_f, C.c_int64, C.c_int, c_f, c_f, c_f]),
+    "snb_composite_backward_weights": (C.c_int, [c_f, c_f, c_f, c_f, C.c_float, c_f, C.c_int64, C.c_int, c_f, c_f, c_f]),
+    "snb_field_backward_sigma": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, c_f, C.c_int64,
+                                           c_f, c_f, c_f, c_f]),
+    "snb_field_backward16_sigma": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, C.c_int64, c_f,
+                                             c_f, c_f]),
 }
 BWD_WS_FLOATS = 2 * 128 * 256 + 128   # SNB_BWD_WS_FLOATS
 

@@ -50,21 +50,25 @@ int launch_importance_merge(const float*, const float*, const float*, int64_t, i
                             float*, cudaStream_t);
 int field_forward_fp32(const void*, const float*, const float*, int64_t, int, int, float*, cudaStream_t);
 int mlp_forward_fp32(const void*, const float*, int64_t, int64_t, int, float*, cudaStream_t);
-int field_forward_train_fp32(const void*, const float*, const float*, int64_t, int, float*, float*, float*, float*,
+int field_forward_train_fp32(const void*, const float*, const float*, int64_t, int, int, float*, float*, float*, float*,
                              float*, cudaStream_t);
-int launch_composite_bwd(const float*, const float*, const float*, const float*, float, int, const float*,
+int launch_composite_bwd(const float*, int, const float*, const float*, const float*, float, int, const float*,
                          const float*, const float*, int64_t, int, float*, const SnbLossSpec*, const float*,
                          const float*, const float*, float*, cudaStream_t);
 int field_backward_fp32(const float* const*, float* const*, int, const float*, const float*, const float*,
                         const float*, const float*, const float*, int64_t, float*, float*, float*, float*,
                         uint32_t*, cudaStream_t);
+int field_backward_sigma_fp32(const float* const*, float* const*, const float*, const float*, const float*, int64_t, float*,
+                              float*, uint32_t*, cudaStream_t);
 int launch_generate_rays(const float*, float, float, float, float, float, float, int, int, int, int, int, int, float*,
                          cudaStream_t);
-int field_forward_train16_tc(const void*, int, const float*, const float*, int64_t, int, float*, void*, cudaStream_t);
+int field_forward_train16_tc(const void*, int, const float*, const float*, int64_t, int, int, float*, void*, cudaStream_t);
 size_t act16_bytes(long long);
 size_t bwd16_workspace_bytes(long long);
 int field_backward16(const float* const*, float* const*, int, const float*, const float*, const void*, long long, void*,
                      const float*, cudaStream_t);
+int field_backward16_sigma(const float* const*, float* const*, const float*, const void*, long long, void*, const float*,
+                           cudaStream_t);
 int adam_step_pack(float* const*, const float* const*, float*, float*, const SnbAdamArgs&, int, int, void*, cudaStream_t);
 int optim_step_pack(float* const*, const float* const*, float*, float*, float*, const SnbOptimArgs&, int, int, void*,
                     cudaStream_t);
@@ -72,7 +76,7 @@ int optim_step_pack(float* const*, const float* const*, float*, float*, float*, 
 size_t tc_packed_bytes(int precision);
 int field_forward_tc(const void*, int, const float*, const float*, int64_t, int, int, float*, cudaStream_t);
 int mlp_forward_tc(const void*, int, const float*, int64_t, int64_t, int, float*, cudaStream_t);
-int field_forward_train_tc(const void*, int, const float*, const float*, int64_t, int, float*, float*, float*, float*,
+int field_forward_train_tc(const void*, int, const float*, const float*, int64_t, int, int, float*, float*, float*, float*,
                            float*, cudaStream_t);
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
@@ -275,9 +279,25 @@ int snb_field_forward_train(const void* packed, int precision, const float* rays
               "snb_field_forward_train: buffers must be 16-byte aligned");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (precision == SNB_PREC_FP32)
-    return field_forward_train_fp32(packed, rays, z_vals, n_rays, n_samples, raw, save_enc, save_dir, save_h, save_g, st);
-  return field_forward_train_tc(packed, precision, rays, z_vals, n_rays, n_samples, raw, save_enc, save_dir, save_h,
+    return field_forward_train_fp32(packed, rays, z_vals, n_rays, n_samples, 0, raw, save_enc, save_dir, save_h, save_g, st);
+  return field_forward_train_tc(packed, precision, rays, z_vals, n_rays, n_samples, 0, raw, save_enc, save_dir, save_h,
                                 save_g, st);
+}
+
+int snb_field_forward_train_sigma(const void* packed, int precision, const float* rays, const float* z_vals,
+                                  int64_t n_rays, int n_samples, float* sigma, float* save_enc, float* save_h,
+                                  void* stream) {
+  if (int rc = check_precision(precision)) return rc;
+  SNB_REQUIRE(n_rays >= 0 && n_samples >= 1, "snb_field_forward_train_sigma: bad extents");
+  SNB_REQUIRE(n_rays == 0 || (packed && rays && z_vals && sigma && save_enc && save_h),
+              "snb_field_forward_train_sigma: null pointer");
+  SNB_REQUIRE(aligned16(rays) && aligned16(save_enc) && aligned16(save_h),
+              "snb_field_forward_train_sigma: rays / save_enc / save_h must be 16-byte aligned");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (precision == SNB_PREC_FP32)
+    return field_forward_train_fp32(packed, rays, z_vals, n_rays, n_samples, 1, sigma, save_enc, nullptr, save_h, nullptr, st);
+  return field_forward_train_tc(packed, precision, rays, z_vals, n_rays, n_samples, 1, sigma, save_enc, nullptr, save_h,
+                                nullptr, st);
 }
 
 int snb_composite_backward(const float* raw, const float* z_vals, const float* rays, const float* noise,
@@ -287,9 +307,19 @@ int snb_composite_backward(const float* raw, const float* z_vals, const float* r
   SNB_REQUIRE(n_rays == 0 || (raw && z_vals && rays && g_raw), "snb_composite_backward: null pointer");
   SNB_REQUIRE(aligned16(raw) && aligned16(g_raw), "snb_composite_backward: raw / g_raw must be 16-byte aligned");
   const float* nz = (noise_std != 0.f) ? noise : nullptr;
-  return launch_composite_bwd(raw, z_vals, rays, nz, noise_std, white_back, g_rgb, g_depth, g_weights, n_rays,
+  return launch_composite_bwd(raw, 4, z_vals, rays, nz, noise_std, white_back, g_rgb, g_depth, g_weights, n_rays,
                               n_samples, g_raw, nullptr, nullptr, nullptr, nullptr, nullptr,
                               reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_composite_backward_weights(const float* sigma, const float* z_vals, const float* rays, const float* noise,
+                                   float noise_std, const float* g_weights, int64_t n_rays, int n_samples,
+                                   float* g_sigma, float* g_amax, void* stream) {
+  SNB_REQUIRE(n_rays >= 0 && n_samples >= 1, "snb_composite_backward_weights: bad extents");
+  SNB_REQUIRE(n_rays == 0 || (sigma && z_vals && rays && g_weights && g_sigma), "snb_composite_backward_weights: null pointer");
+  const float* nz = (noise_std != 0.f) ? noise : nullptr;
+  return launch_composite_bwd(sigma, 1, z_vals, rays, nz, noise_std, 0, nullptr, nullptr, g_weights, n_rays, n_samples,
+                              g_sigma, nullptr, nullptr, nullptr, nullptr, g_amax, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_composite_backward_loss(const float* raw, const float* z_vals, const float* rays, const float* noise,
@@ -306,7 +336,7 @@ int snb_composite_backward_loss(const float* raw, const float* z_vals, const flo
                 "snb_composite_backward_loss: the forward's rgb / depth outputs are required with a loss spec");
   }
   const float* nz = (noise_std != 0.f) ? noise : nullptr;
-  return launch_composite_bwd(raw, z_vals, rays, nz, noise_std, white_back, g_rgb, g_depth, g_weights, n_rays,
+  return launch_composite_bwd(raw, 4, z_vals, rays, nz, noise_std, white_back, g_rgb, g_depth, g_weights, n_rays,
                               n_samples, g_raw, loss, rgb, depth, g_loss, g_amax, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -324,6 +354,23 @@ int snb_field_backward(const float* const* params, float* const* grads, int new_
                              n_points, ws_a, ws_b, ws_s, ws_w, ws_m, reinterpret_cast<cudaStream_t>(stream));
 }
 
+// the tensors a sigma-only pass reads: layers 1-8 and the sigma head
+static bool sigma_pass_tensor(int i) { return i < 16 || i == 20 || i == 21; }
+
+int snb_field_backward_sigma(const float* const* params, float* const* grads, const float* g_sigma,
+                             const float* save_enc, const float* save_h, int64_t n_points, float* ws_a, float* ws_b,
+                             uint32_t* ws_m, void* stream) {
+  SNB_REQUIRE(n_points >= 0, "snb_field_backward_sigma: negative point count");
+  SNB_REQUIRE(params && grads, "snb_field_backward_sigma: null parameter arrays");
+  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i)
+    SNB_REQUIRE(!sigma_pass_tensor(i) || (params[i] && grads[i]), "snb_field_backward_sigma: parameter / gradient tensor %d is null", i);
+  SNB_REQUIRE(n_points == 0 || (g_sigma && save_enc && save_h && ws_a && ws_b && ws_m), "snb_field_backward_sigma: null pointer");
+  SNB_REQUIRE(aligned16(save_enc) && aligned16(save_h) && aligned16(ws_a) && aligned16(ws_b) && aligned16(ws_m),
+              "snb_field_backward_sigma: save_enc / save_h / scratch must be 16-byte aligned");
+  return field_backward_sigma_fp32(params, grads, g_sigma, save_enc, save_h, n_points, ws_a, ws_b, ws_m,
+                                   reinterpret_cast<cudaStream_t>(stream));
+}
+
 size_t snb_act16_bytes(int64_t n_points) { return n_points < 0 ? 0 : act16_bytes(n_points); }
 size_t snb_bwd16_workspace_bytes(int64_t n_points) { return n_points < 0 ? 0 : bwd16_workspace_bytes(n_points); }
 
@@ -336,7 +383,20 @@ int snb_field_forward_train16(const void* packed, int precision, const float* ra
   SNB_REQUIRE(n_rays == 0 || (packed && rays && z_vals && raw && act16), "snb_field_forward_train16: null pointer");
   SNB_REQUIRE(aligned16(rays) && aligned16(raw) && (reinterpret_cast<uintptr_t>(act16) & 255u) == 0,
               "snb_field_forward_train16: rays / raw must be 16-byte and act16 256-byte aligned");
-  return field_forward_train16_tc(packed, precision, rays, z_vals, n_rays, n_samples, raw, act16,
+  return field_forward_train16_tc(packed, precision, rays, z_vals, n_rays, n_samples, 0, raw, act16,
+                                  reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_field_forward_train16_sigma(const void* packed, int precision, const float* rays, const float* z_vals,
+                                    int64_t n_rays, int n_samples, float* sigma, void* act16, void* stream) {
+  if (int rc = check_precision(precision)) return rc;
+  if (precision == SNB_PREC_FP32)
+    return fail(SNB_ERR_UNSUPPORTED, "snb_field_forward_train16_sigma: 16-bit activation storage needs a tensor-core precision mode");
+  SNB_REQUIRE(n_rays >= 0 && n_samples >= 1, "snb_field_forward_train16_sigma: bad extents");
+  SNB_REQUIRE(n_rays == 0 || (packed && rays && z_vals && sigma && act16), "snb_field_forward_train16_sigma: null pointer");
+  SNB_REQUIRE(aligned16(rays) && (reinterpret_cast<uintptr_t>(act16) & 255u) == 0,
+              "snb_field_forward_train16_sigma: rays must be 16-byte and act16 256-byte aligned");
+  return field_forward_train16_tc(packed, precision, rays, z_vals, n_rays, n_samples, 1, sigma, act16,
                                   reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -353,6 +413,19 @@ int snb_field_backward16(const float* const* params, float* const* grads, int ne
               "snb_field_backward16: g_raw / raw must be 16-byte, act16 / workspace 256-byte aligned");
   return field_backward16(params, grads, new_activation, g_raw, raw, act16, n_points, workspace, g_amax,
                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_field_backward16_sigma(const float* const* params, float* const* grads, const float* g_sigma, const void* act16,
+                               int64_t n_points, void* workspace, const float* g_amax, void* stream) {
+  SNB_REQUIRE(n_points >= 0, "snb_field_backward16_sigma: negative point count");
+  SNB_REQUIRE(params && grads, "snb_field_backward16_sigma: null parameter arrays");
+  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i)
+    SNB_REQUIRE(!sigma_pass_tensor(i) || (params[i] && grads[i]), "snb_field_backward16_sigma: parameter / gradient tensor %d is null", i);
+  SNB_REQUIRE(n_points == 0 || (g_sigma && act16 && workspace), "snb_field_backward16_sigma: null pointer");
+  SNB_REQUIRE((reinterpret_cast<uintptr_t>(act16) & 255u) == 0 && (reinterpret_cast<uintptr_t>(workspace) & 255u) == 0,
+              "snb_field_backward16_sigma: act16 / workspace must be 256-byte aligned");
+  return field_backward16_sigma(params, grads, g_sigma, act16, n_points, workspace, g_amax,
+                                reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_adam_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,

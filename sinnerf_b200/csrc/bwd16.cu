@@ -12,6 +12,9 @@
 //   dir layer : dW', db' = wgrad16(dS, h8) with the sigma-head rows riding on the same X operand (dW_sigma = hg[3]^T h8);
 //               dWd[:, 256:] = wgrad16(dS, dir);  dW_rgb = hg[0..2]^T g;  unfold through W'
 //   layers    : dH_{l-1} = dgrad16(dH_l, W_l) * mask(h_l);  dW_l, db_l = wgrad16(dH_l, h_l)          l = 8 .. 1
+// A sigma-only pass (field_backward16_sigma) replaces the heads and the direction layer by sigma_head_bwd16_kernel
+// (dH8 and the head-gradient cell straight from g_sigma) and the head rows of wgrad16 (dW_sigma), then walks the
+// same layers (trunk_backward16).
 // HBM per point: ~2.5 KB per 256-wide layer (fp32 version: ~5 KB), 4.5 KB of saved activations (8.9 KB).
 #include <cuda_fp16.h>
 
@@ -33,12 +36,10 @@ namespace {
 // ------------------------------------------------------------------------------------------
 // max |g_raw| when the compositing backward did not provide it (stand-alone use of the C ABI)
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) amax_kernel(const float4* __restrict__ g, long long n, uint32_t* __restrict__ out) {
+__global__ void __launch_bounds__(256) amax_kernel(const float* __restrict__ g, long long n, uint32_t* __restrict__ out) {
   float m = 0.f;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float4 v = g[i];
-    m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
-  }
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    m = fmaxf(m, fabsf(g[i]));
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
   if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_uint(m == m ? fminf(m, 3.0e38f) : 3.0e38f));
@@ -77,7 +78,8 @@ __global__ void __launch_bounds__(256) bwd16_prepare_kernel(PrepArgs a) {
     else {
       a.state[ST_EVEC_MAX] = m;
       float wr = 0.f;
-      for (int j = 0; j < kHalf; ++j) wr = fmaxf(wr, fabsf(a.w_rgb[j]) + fabsf(a.w_rgb[kHalf + j]) + fabsf(a.w_rgb[2 * kHalf + j]));
+      for (int j = 0; a.w_rgb != nullptr && j < kHalf; ++j)
+        wr = fmaxf(wr, fabsf(a.w_rgb[j]) + fabsf(a.w_rgb[kHalf + j]) + fabsf(a.w_rgb[2 * kHalf + j]));
       a.state[ST_WR_L1] = wr;
       if (a.g_amax != nullptr) reinterpret_cast<uint32_t*>(a.state)[ST_AMAX_G] = *a.g_amax;
     }
@@ -186,7 +188,88 @@ __global__ void __launch_bounds__(256) head_bwd16_kernel(Head16Args a) {
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// sigma head of a sigma-only pass: g_sigma (P,) is all that flows in.  A warp walks 32-point tiles, lane = point;
+// it reads g_sigma and h8's 8 ReLU mask words and writes the 32 cells of dH8 (hi + residual planes) and the
+// head-gradient cell [0, 0, 0, g_sigma | residuals] that the head rows of wgrad16 turn into dW_sigma.
+//   dH8_j = g_sigma w_sigma[j] [h8_j > 0];   db_sigma += g_sigma
+// Scales: |dH8| <= max |g_sigma| max |w_sigma| (rigorous), |hg| <= max |g_sigma|; both powers of two are chosen here
+// from the two device scalars, so no host round trip.
+// ------------------------------------------------------------------------------------------
+struct SigmaHead16Args {
+  const float* g_sigma;      // (P,)
+  const uint32_t* mask;      // (8 words, Ppad): the ReLU mask of h8
+  const float* ws;           // (256) sigma head weights
+  unsigned char* dH;         // (Ppad,256) fp16 T32, scaled by state[ST_SCALE_H0 + 7]
+  unsigned char* dH_lo;      // residual plane
+  unsigned char* hg;         // (Ppad,8) fp16 T32, scaled by state[ST_SCALE_HG]
+  float* dbs;
+  float* state;
+  long long P, ppad;
+};
+
+__global__ void __launch_bounds__(256) sigma_head_bwd16_kernel(SigmaHead16Args a) {
+  __shared__ float wsig[kWidth];
+  const int tid = threadIdx.x, lane = tid & 31;
+  for (int j = tid; j < kWidth; j += blockDim.x) wsig[j] = a.ws[j];
+  __syncthreads();
+  const float amax_g = __uint_as_float(reinterpret_cast<const uint32_t*>(a.state)[ST_AMAX_G]);
+  const float s_hg = pow2_scale(amax_g, kA16Target);
+  const float s_h = pow2_scale(amax_g * a.state[ST_EVEC_MAX], kA16Target);
+  if (blockIdx.x == 0 && tid == 0) { a.state[ST_SCALE_HG] = s_hg; a.state[ST_SCALE_H0 + 7] = s_h; }
+  const long long warp = ((long long)blockIdx.x * blockDim.x + tid) >> 5;
+  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  float abs_ = 0.f, amax = 0.f;
+  for (long long tile = warp; tile * 32 < a.ppad; tile += nwarps) {
+    const long long p = tile * 32 + lane;
+    const bool live = p < a.P;
+    const float gs = live ? a.g_sigma[p] : 0.f;
+    abs_ += gs;
+    {
+      const float hv = gs * s_hg;
+      const uint32_t h23 = pack_half2_sat(0.f, hv);
+      const float2 f23 = __half22float2(*reinterpret_cast<const __half2*>(&h23));
+      *reinterpret_cast<uint4*>(a.hg + a16_cell(p, 0, 8)) = make_uint4(0u, h23, 0u, pack_half2_sat(0.f, hv - f23.y));
+    }
+    const float gsc = gs * s_h;
+#pragma unroll 2
+    for (int wd = 0; wd < 8; ++wd) {
+      const uint32_t m = live ? __ldg(a.mask + (size_t)wd * (size_t)a.ppad + p) : 0u;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int f8 = 4 * wd + q;
+        uint32_t o[4], ol[4];
+#pragma unroll
+        for (int j2 = 0; j2 < 4; ++j2) {
+          const int c = 8 * q + 2 * j2;           // bit of the word = feature 32 wd + c
+          const float x0 = (m >> c) & 1u ? gsc * wsig[8 * f8 + 2 * j2] : 0.f;
+          const float x1 = (m >> (c + 1)) & 1u ? gsc * wsig[8 * f8 + 2 * j2 + 1] : 0.f;
+          amax = fmaxf(amax, fmaxf(fabsf(x0), fabsf(x1)));
+          o[j2] = pack_half2_sat(x0, x1);
+          const float2 hv = __half22float2(*reinterpret_cast<const __half2*>(&o[j2]));
+          ol[j2] = pack_half2_sat(x0 - hv.x, x1 - hv.y);
+        }
+        *reinterpret_cast<uint4*>(a.dH + a16_cell(p, f8, kWidth)) = make_uint4(o[0], o[1], o[2], o[3]);
+        *reinterpret_cast<uint4*>(a.dH_lo + a16_cell(p, f8, kWidth)) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+      }
+    }
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    abs_ += __shfl_xor_sync(0xffffffffu, abs_, off);
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, off));
+  }
+  if (lane == 0) {
+    atomicAdd(a.dbs, abs_);
+    if (amax > 0.f)
+      atomicMax(reinterpret_cast<uint32_t*>(a.state) + ST_AMAX_H0 + 7, __float_as_uint(amax == amax ? fminf(amax, 65504.f) : 65504.f));
+  }
+}
+
 }  // namespace
+
+static int trunk_backward16(const float* const* params, float* const* grads, const unsigned char* act, unsigned char* w,
+                            float* state, long long P, cudaStream_t st);
 
 size_t act16_bytes(long long n_points) { return make_act16_layout(n_points).total; }
 size_t bwd16_workspace_bytes(long long n_points) { return make_bwd16_layout(n_points).total; }
@@ -212,7 +295,7 @@ int field_backward16(const float* const* params, float* const* grads, int new_ac
   if (cudaMemsetAsync(state, 0, kBwdStateFloats * sizeof(float), st) != cudaSuccess)
     return fail(SNB_ERR_CUDA, "field_backward16: cudaMemsetAsync failed");
   if (g_amax == nullptr) {
-    amax_kernel<<<sm_count() * 4, 256, 0, st>>>(reinterpret_cast<const float4*>(g_raw), P, reinterpret_cast<uint32_t*>(state) + ST_AMAX_G);
+    amax_kernel<<<sm_count() * 4, 256, 0, st>>>(g_raw, 4 * P, reinterpret_cast<uint32_t*>(state) + ST_AMAX_G);
     if ((rc = check_launch("amax_kernel"))) return rc;
   }
   if ((rc = launch_fold_weights(params[18], params[16], fold, st))) return rc;
@@ -252,13 +335,77 @@ int field_backward16(const float* const* params, float* const* grads, int new_ac
   }
   if ((rc = launch_unfold_grads(params[18], params[16], params[17], fold, grads[18], grads[19], grads[16], grads[17], st))) return rc;
   // into h8: through W', plus the sigma head's term; ReLU mask of h8
+  if ((rc = run_dgrad16(w + B.ds, w + B.ds_lo, 128, fold + kFoldW, 256, 0, M(7), g_raw + 3, 4, params[kSigmaW], w + B.dya,
+                        w + B.dya_lo, state, ST_AMAX_DS, ST_SCALE_DS, ST_L1_FOLD, ST_AMAX_H0 + 7, ST_SCALE_H0 + 7, P, st)))
+    return rc;
+  return trunk_backward16(params, grads, act, w, state, P, st);
+}
+
+// Backward of a sigma-only pass: g_sigma (P,) -> the gradients of layers 1-8 and the sigma head (grads 0..15, 20, 21;
+// the others are not touched).  The sigma head kernel forms dH8 directly; from there on it is the full pass's chain.
+int field_backward16_sigma(const float* const* params, float* const* grads, const float* g_sigma, const void* act16,
+                           long long P, void* ws, const float* g_amax, cudaStream_t st) {
+  if (P == 0) return SNB_OK;
+  const long long ppad = a16_pad(P);
+  const Act16Layout A = make_act16_layout(P);
+  const Bwd16Layout B = make_bwd16_layout(P);
+  const unsigned char* act = reinterpret_cast<const unsigned char*>(act16);
+  unsigned char* w = reinterpret_cast<unsigned char*>(ws);
+  float* state = reinterpret_cast<float*>(w + B.state);
+  int rc;
+  if (cudaMemsetAsync(state, 0, kBwdStateFloats * sizeof(float), st) != cudaSuccess)
+    return fail(SNB_ERR_CUDA, "field_backward16_sigma: cudaMemsetAsync failed");
+  if (g_amax == nullptr) {
+    amax_kernel<<<sm_count() * 4, 256, 0, st>>>(g_sigma, P, reinterpret_cast<uint32_t*>(state) + ST_AMAX_G);
+    if ((rc = check_launch("amax_kernel"))) return rc;
+  }
+  {
+    // the trunk's column norms and max |w_sigma|; there is no W' (block 0 re-measures W_1, unused) and no rgb head
+    PrepArgs a{};
+    for (int l = 0; l < 8; ++l) {
+      const int m = l == 0 ? 1 : l;
+      a.W[l] = params[2 * m]; a.rows[l] = kWidth; a.ldw[l] = m == 4 ? 319 : 256; a.col_off[l] = m == 4 ? kXyzCh : 0;
+    }
+    a.w_sigma = params[kSigmaW]; a.w_rgb = nullptr;
+    a.g_amax = reinterpret_cast<const uint32_t*>(g_amax);
+    a.state = state;
+    bwd16_prepare_kernel<<<9, 256, 0, st>>>(a);
+    if ((rc = check_launch("bwd16_prepare_kernel"))) return rc;
+  }
+  {
+    SigmaHead16Args a{g_sigma, reinterpret_cast<const uint32_t*>(act + A.mask) + (size_t)7 * 8 * (size_t)ppad, params[kSigmaW],
+                      w + B.dya, w + B.dya_lo, w + B.hg, grads[kSigmaB], state, P, ppad};
+    long long tiles = ppad / 32, blocks = (tiles + 7) / 8;
+    if (blocks > sm_count() * 4) blocks = sm_count() * 4;
+    sigma_head_bwd16_kernel<<<(unsigned)blocks, 256, 0, st>>>(a);
+    if ((rc = check_launch("sigma_head_bwd16_kernel"))) return rc;
+  }
+  {
+    // dW_sigma = hg[3]^T h8: the head rows of wgrad16 alone
+    float* dH[8] = {nullptr, nullptr, nullptr, grads[kSigmaW], nullptr, nullptr, nullptr, nullptr};
+    const float* sc_hg = state + ST_SCALE_HG;
+    if ((rc = run_wgrad16(nullptr, 0, act + A.h[7], 256, 256, nullptr, 0, 0, nullptr, sc_hg, w + B.hg, dH, sc_hg, ppad, st)))
+      return rc;
+  }
+  return trunk_backward16(params, grads, act, w, state, P, st);
+}
+
+// The trunk from dH8 down, shared by both drivers.  On entry dH8 is in the workspace's dYa planes (hi + residual) with
+// its scale in state[ST_SCALE_H0 + 7] and its running max in state[ST_AMAX_H0 + 7].
+//   dH_{l-1} = dgrad16(dH_l, W_l) * mask(h_{l-1});  dW_l, db_l = wgrad16(dH_l, h_{l-1})      l = 8 .. 2;  then layer 1
+static int trunk_backward16(const float* const* params, float* const* grads, const unsigned char* act, unsigned char* w,
+                            float* state, long long P, cudaStream_t st) {
+  const long long ppad = a16_pad(P);
+  const Act16Layout A = make_act16_layout(P);
+  const Bwd16Layout B = make_bwd16_layout(P);
+  const uint32_t* mask = reinterpret_cast<const uint32_t*>(act + A.mask);
+  auto H = [&](int l) { return act + A.h[l]; };                          // l = 0..7: h1..h8
+  auto M = [&](int l) { return mask + (size_t)l * 8 * (size_t)ppad; };   // ReLU mask of h_{l+1}
+  int rc;
   unsigned char* cur = w + B.dya;
   unsigned char* nxt = w + B.dyb;
   unsigned char* cur_lo = w + B.dya_lo;
   unsigned char* nxt_lo = w + B.dyb_lo;
-  if ((rc = run_dgrad16(w + B.ds, w + B.ds_lo, 128, fold + kFoldW, 256, 0, M(7), g_raw + 3, 4, params[kSigmaW], cur,
-                        cur_lo, state, ST_AMAX_DS, ST_SCALE_DS, ST_L1_FOLD, ST_AMAX_H0 + 7, ST_SCALE_H0 + 7, P, st)))
-    return rc;
   for (int l = 7; l >= 1; --l) {
     const int ldw = l == 4 ? 319 : 256;
     const float* sc = state + ST_SCALE_H0 + l;

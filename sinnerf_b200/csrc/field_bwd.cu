@@ -9,7 +9,8 @@
 //   per layer : dW_l += dY_l^T X_l, db_l += sum dY_l                            (run_wgrad_tc)
 //               dX_l  = dY_l W_l  (x ReLU mask of the saved input, + sigma term at h8)   (run_dgrad_tc)
 // walking dir layer -> layers 8..1.  Nothing flows into rays, z or across sample_pdf (the reference
-// detaches it, models/rendering.py:311-313).
+// detaches it, models/rendering.py:311-313).  A sigma-only pass starts at dH8 (sigma_head_bwd_kernel) and walks
+// the same layers (trunk_backward_fp32).
 //
 // Activations are plain (P, C) row-major fp32 tensors.  The wgrad of a layer also leaves [X > 0] as bit words
 // (ws_m) for the dgrad of the same layer, which applies them as the ReLU mask.
@@ -175,6 +176,81 @@ int launch_unfold_grads(const float* Wd, const float* Wf, const float* bf, const
   return check_launch("unfold_grads_kernel");
 }
 
+// ------------------------------------------------------------------------------------------
+// sigma head of a sigma-only pass (render_rays(test_time=True)'s coarse pass, eval_points): g_sigma (P,) is all that
+// flows in.  One warp walks points, a lane owns 8 of the 256 trunk units:
+//   dH8 = g_sigma w_sigma * [h8 > 0];   dW_sigma += g_sigma h8;   db_sigma += g_sigma
+// ------------------------------------------------------------------------------------------
+struct SigmaHeadArgs {
+  const float* g_sigma;  // (P,)
+  const float* H8;       // (P,256)
+  const float* ws;       // (256) sigma head weights
+  float* dH;             // (P,256)
+  float* dWs; float* dbs;
+  long long P;
+};
+
+__global__ void __launch_bounds__(256) sigma_head_bwd_kernel(SigmaHeadArgs a) {
+  const int lane = threadIdx.x & 31;
+  const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  float w[8], aws[8] = {}, abs_ = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) w[j] = a.ws[lane * 8 + j];
+  constexpr int kU = 4;          // 4 points per warp iteration, loads first (as head_bwd_kernel)
+  for (long long pb = warp * kU; pb < a.P; pb += nwarps * kU) {
+    float g[kU];
+    float4 h0[kU], h1[kU];
+#pragma unroll
+    for (int u = 0; u < kU; ++u) {
+      const long long p = pb + u < a.P ? pb + u : a.P - 1;
+      g[u] = a.g_sigma[p];
+      h0[u] = *reinterpret_cast<const float4*>(a.H8 + p * 256 + lane * 8);
+      h1[u] = *reinterpret_cast<const float4*>(a.H8 + p * 256 + lane * 8 + 4);
+    }
+#pragma unroll
+    for (int u = 0; u < kU; ++u) {
+      if (pb + u >= a.P) break;
+      const long long p = pb + u;
+      const float hv[8] = {h0[u].x, h0[u].y, h0[u].z, h0[u].w, h1[u].x, h1[u].y, h1[u].z, h1[u].w};
+      float d[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        d[j] = hv[j] > 0.f ? g[u] * w[j] : 0.f;
+        aws[j] = fmaf(g[u], hv[j], aws[j]);
+      }
+      *reinterpret_cast<float4*>(a.dH + p * 256 + lane * 8) = make_float4(d[0], d[1], d[2], d[3]);
+      *reinterpret_cast<float4*>(a.dH + p * 256 + lane * 8 + 4) = make_float4(d[4], d[5], d[6], d[7]);
+      if (lane == 0) abs_ += g[u];
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) atomicAdd(a.dWs + lane * 8 + j, aws[j]);
+  if (lane == 0) atomicAdd(a.dbs, abs_);
+}
+
+// The trunk from dH8 (in cur, (P,256)) down: trunk layers 8..2 (index l = 7..1), dY lives in cur, dX goes to nxt;
+// then layer 1's weights.  Shared by the full and the sigma-only pass.
+static int trunk_backward_fp32(const float* const* params, float* const* grads, const float* save_enc,
+                               const float* save_h, float* cur, float* nxt, uint32_t* ws_m, long long P, cudaStream_t st) {
+  auto H = [&](int l) { return save_h + (size_t)l * P * kWidth; };   // l = 0..7: h1..h8
+  int rc;
+  for (int l = 7; l >= 1; --l) {
+    const int ldw = l == 4 ? 319 : 256;
+    if (l == 4) {
+      if ((rc = run_wgrad_tc(cur, 256, save_enc, kXyzPad, kXyzCh, grads[2 * l], ldw, 0, grads[2 * l + 1], nullptr, P, st))) return rc;
+      if ((rc = run_wgrad_tc(cur, 256, H(l - 1), 256, 256, grads[2 * l], ldw, kXyzCh, nullptr, ws_m, P, st))) return rc;
+      if ((rc = run_dgrad_tc(cur, 256, params[2 * l], ldw, kXyzCh, ws_m, nullptr, 0, nullptr, nxt, P, st))) return rc;
+    } else {
+      if ((rc = run_wgrad_tc(cur, 256, H(l - 1), 256, 256, grads[2 * l], ldw, 0, grads[2 * l + 1], ws_m, P, st))) return rc;
+      if ((rc = run_dgrad_tc(cur, 256, params[2 * l], ldw, 0, ws_m, nullptr, 0, nullptr, nxt, P, st))) return rc;
+    }
+    float* t = cur; cur = nxt; nxt = t;
+  }
+  // layer 1: weights only
+  return run_wgrad_tc(cur, 256, save_enc, kXyzPad, kXyzCh, grads[0], 63, 0, grads[1], nullptr, P, st);
+}
+
 // params / grads: 24 device pointers in state-dict order (SNB_N_PARAM_TENSORS); grads are accumulated into.
 int field_backward_fp32(const float* const* params, float* const* grads, int new_activation, const float* g_raw,
                         const float* raw, const float* save_enc, const float* save_dir, const float* save_h,
@@ -200,23 +276,20 @@ int field_backward_fp32(const float* const* params, float* const* grads, int new
     return rc;
   // into h8: through W', plus the sigma head's term; ReLU mask of h8
   if ((rc = run_dgrad_tc(ws_s, 128, ws_w + kFoldW, 256, 0, ws_m, g_raw + 3, 4, params[kSigmaW], ws_b, P, st))) return rc;
-  // trunk layers 8..2 (index l = 7..1): dY lives in cur, dX goes to nxt
-  float* cur = ws_b;
-  float* nxt = ws_a;
-  for (int l = 7; l >= 1; --l) {
-    const int ldw = l == 4 ? 319 : 256;
-    if (l == 4) {
-      if ((rc = run_wgrad_tc(cur, 256, save_enc, kXyzPad, kXyzCh, grads[2 * l], ldw, 0, grads[2 * l + 1], nullptr, P, st))) return rc;
-      if ((rc = run_wgrad_tc(cur, 256, H(l - 1), 256, 256, grads[2 * l], ldw, kXyzCh, nullptr, ws_m, P, st))) return rc;
-      if ((rc = run_dgrad_tc(cur, 256, params[2 * l], ldw, kXyzCh, ws_m, nullptr, 0, nullptr, nxt, P, st))) return rc;
-    } else {
-      if ((rc = run_wgrad_tc(cur, 256, H(l - 1), 256, 256, grads[2 * l], ldw, 0, grads[2 * l + 1], ws_m, P, st))) return rc;
-      if ((rc = run_dgrad_tc(cur, 256, params[2 * l], ldw, 0, ws_m, nullptr, 0, nullptr, nxt, P, st))) return rc;
-    }
-    float* t = cur; cur = nxt; nxt = t;
-  }
-  // layer 1: weights only
-  return run_wgrad_tc(cur, 256, save_enc, kXyzPad, kXyzCh, grads[0], 63, 0, grads[1], nullptr, P, st);
+  return trunk_backward_fp32(params, grads, save_enc, save_h, ws_b, ws_a, ws_m, P, st);
+}
+
+// Backward of a sigma-only pass: g_sigma (P,) -> the gradients of layers 1-8 and the sigma head (grads 0..15, 20, 21;
+// the others are not touched).  Scratch: ws_a, ws_b (P,256), ws_m (P,8).
+int field_backward_sigma_fp32(const float* const* params, float* const* grads, const float* g_sigma,
+                              const float* save_enc, const float* save_h, int64_t n_points, float* ws_a, float* ws_b,
+                              uint32_t* ws_m, cudaStream_t st) {
+  const long long P = n_points;
+  if (P == 0) return SNB_OK;
+  SigmaHeadArgs a{g_sigma, save_h + (size_t)7 * P * kWidth, params[kSigmaW], ws_b, grads[kSigmaW], grads[kSigmaB], P};
+  sigma_head_bwd_kernel<<<sm_count() * 4, 256, 0, st>>>(a);
+  if (int rc = check_launch("sigma_head_bwd_kernel")) return rc;
+  return trunk_backward_fp32(params, grads, save_enc, save_h, ws_b, ws_a, ws_m, P, st);
 }
 
 }  // namespace snb

@@ -238,7 +238,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) field_simt_kernel(FieldParams p) 
         const int r = e / 96, k = e - r * 96;
         if (p0 + r < p.n_points) {
           if (k < kXyzPad) p.save_enc[(p0 + r) * kXyzPad + k] = s.enc[aidx(k, r)];
-          else p.save_dir[(p0 + r) * kDirPad + (k - kXyzPad)] = s.dir[aidx(k - kXyzPad, r)];
+          else if (p.save_dir != nullptr) p.save_dir[(p0 + r) * kDirPad + (k - kXyzPad)] = s.dir[aidx(k - kXyzPad, r)];
         }
       }
     }
@@ -318,8 +318,9 @@ static int launch_field_simt(const FieldParams& p, cudaStream_t st) {
   return check_launch("field_simt_kernel");
 }
 
+// sigma_only: raw is (P,) sigma and save_dir / save_g are not written (may be NULL)
 int field_forward_train_fp32(const void* packed, const float* rays, const float* z, int64_t n_rays, int n_samples,
-                             float* raw, float* save_enc, float* save_dir, float* save_h, float* save_g,
+                             int sigma_only, float* raw, float* save_enc, float* save_dir, float* save_h, float* save_g,
                              cudaStream_t st) {
   FieldParams p{};
   p.hdr = reinterpret_cast<const PackedHeader*>(packed);
@@ -327,7 +328,7 @@ int field_forward_train_fp32(const void* packed, const float* rays, const float*
   p.z = z;
   p.n_samples = n_samples;
   p.n_points = (long long)n_rays * n_samples;
-  p.sigma_only = 0;
+  p.sigma_only = sigma_only;
   p.out = raw;
   p.save_enc = save_enc; p.save_dir = save_dir; p.save_h = save_h; p.save_g = save_g;
   return launch_field_simt<false>(p, st);

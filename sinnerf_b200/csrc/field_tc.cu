@@ -997,13 +997,16 @@ int field_forward_tc(const void* packed, int precision, const float* rays, const
   return dispatch_tc<false>(precision, p, st);
 }
 
+// sigma_only (both training entries): layers 1-8 and the sigma head only; raw is (P,) sigma, the direction encoding
+// and the direction layer's output are neither computed nor stored (save_dir / save_g may be NULL)
 int field_forward_train_tc(const void* packed, int precision, const float* rays, const float* z, int64_t n_rays,
-                           int n_samples, float* raw, float* save_enc, float* save_dir, float* save_h, float* save_g,
-                           cudaStream_t st) {
+                           int n_samples, int sigma_only, float* raw, float* save_enc, float* save_dir, float* save_h,
+                           float* save_g, cudaStream_t st) {
   TcParams p{};
   p.image = reinterpret_cast<const unsigned char*>(packed);
   p.rays = rays; p.z = z; p.n_samples = n_samples;
   p.n_points = (long long)n_rays * n_samples;
+  p.sigma_only = sigma_only;
   p.out = raw;
   p.save_enc = save_enc; p.save_dir = save_dir; p.save_h = save_h; p.save_g = save_g;
   return dispatch_tc<false, 1>(precision, p, st);
@@ -1011,11 +1014,12 @@ int field_forward_train_tc(const void* packed, int precision, const float* rays,
 
 // training forward with 16-bit activation storage (act16.cuh): `act16` = one buffer of make_act16_layout(P).total bytes
 int field_forward_train16_tc(const void* packed, int precision, const float* rays, const float* z, int64_t n_rays,
-                             int n_samples, float* raw, void* act16, cudaStream_t st) {
+                             int n_samples, int sigma_only, float* raw, void* act16, cudaStream_t st) {
   TcParams p{};
   p.image = reinterpret_cast<const unsigned char*>(packed);
   p.rays = rays; p.z = z; p.n_samples = n_samples;
   p.n_points = (long long)n_rays * n_samples;
+  p.sigma_only = sigma_only;
   p.out = raw;
   const Act16Layout L = make_act16_layout(p.n_points);
   unsigned char* b = reinterpret_cast<unsigned char*>(act16);

@@ -318,10 +318,11 @@ __global__ void __launch_bounds__(256) composite_fwd_kernel(
 //   galpha_i = gw_i T_i - (sum_{k>i} gw_k w_k) / (1 - alpha_i + 1e-10)
 //   gsigma_i = galpha_i delta_i exp(-delta_i relu(s_i)) [s_i > 0],   s_i = sigma_i + noise_i
 //   gc_i     = g_rgb w_i
+// raw_channels = 1 is the weights-only pass (rendering.py:237-238): raw and g_raw are (N,S) sigma rows, c_i = 0.
 // Algorithmic bytes: 16+4(+4) in, 16 out per point (+4 if g_w is given).
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) composite_bwd_kernel(
-    const float* __restrict__ raw, const float* __restrict__ z_vals, const float* __restrict__ rays,
+    const float* __restrict__ raw, int raw_channels, const float* __restrict__ z_vals, const float* __restrict__ rays,
     const float* __restrict__ noise, float noise_std, int white_back, const float* __restrict__ g_rgb,
     const float* __restrict__ g_depth, const float* __restrict__ g_w, long long n_rays, int S,
     float* __restrict__ g_raw, LossSpec ls, const float* __restrict__ out_rgb, const float* __restrict__ out_depth,
@@ -360,7 +361,8 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(
       const bool valid = i < S;
       float alpha = 0.f, t = 1.0f, gw = 0.f;
       if (valid) {
-        const float4 v = reinterpret_cast<const float4*>(raw)[ray * S + i];
+        const float4 v = raw_channels == 4 ? reinterpret_cast<const float4*>(raw)[ray * S + i]
+                                           : make_float4(0.f, 0.f, 0.f, raw[ray * S + i]);
         const float z = zr[i];
         float delta = (i + 1 < S) ? __fsub_rn(zr[i + 1], z) : 1e10f;
         delta = __fmul_rn(delta, dnorm);
@@ -401,7 +403,8 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(
     }
     __syncwarp();
     for (int i = lane; i < S; i += 32) {
-      const float4 v = reinterpret_cast<const float4*>(raw)[ray * S + i];
+      const float4 v = raw_channels == 4 ? reinterpret_cast<const float4*>(raw)[ray * S + i]
+                                         : make_float4(0.f, 0.f, 0.f, raw[ray * S + i]);
       const float z = zr[i];
       float delta = (i + 1 < S) ? __fsub_rn(zr[i + 1], z) : 1e10f;
       delta = __fmul_rn(delta, dnorm);
@@ -414,7 +417,8 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(
       const float galpha = gw * T - sg[i] / (__fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f));
       const float e = expf(-__fmul_rn(delta, fmaxf(sgm, 0.f)));
       const float gsig = sgm > 0.f ? galpha * delta * e : 0.f;
-      reinterpret_cast<float4*>(g_raw)[ray * S + i] = make_float4(gr * w, gg * w, gb * w, gsig);
+      if (raw_channels == 4) reinterpret_cast<float4*>(g_raw)[ray * S + i] = make_float4(gr * w, gg * w, gb * w, gsig);
+      else g_raw[ray * S + i] = gsig;
       amax = fmaxf(fmaxf(amax, fabsf(gsig)), fmaxf(fmaxf(fabsf(gr * w), fabsf(gg * w)), fabsf(gb * w)));
     }
     __syncwarp();
@@ -587,7 +591,7 @@ __global__ void __launch_bounds__(256) composite_fwd4_kernel(
 // inside the thread plus a log2(L)-step shuffle scan of the per-thread totals.
 template <int L>
 __global__ void __launch_bounds__(256) composite_bwd4_kernel(
-    const float* __restrict__ raw, const float* __restrict__ z_vals, const float* __restrict__ rays,
+    const float* __restrict__ raw, int raw_channels, const float* __restrict__ z_vals, const float* __restrict__ rays,
     const float* __restrict__ noise, float noise_std, int white_back, const float* __restrict__ g_rgb,
     const float* __restrict__ g_depth, const float* __restrict__ g_w, long long n_rays, int S,
     float* __restrict__ g_raw, LossSpec ls, const float* __restrict__ out_rgb, const float* __restrict__ out_depth,
@@ -608,8 +612,13 @@ __global__ void __launch_bounds__(256) composite_bwd4_kernel(
     const long long p0 = ray * S + 4 * sl;
     if (act) {
       zq = *reinterpret_cast<const float4*>(z_vals + p0);
+      if (raw_channels == 4) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) c[k] = reinterpret_cast<const float4*>(raw)[p0 + k];
+        for (int k = 0; k < 4; ++k) c[k] = reinterpret_cast<const float4*>(raw)[p0 + k];
+      } else {
+        const float4 sq = *reinterpret_cast<const float4*>(raw + p0);
+        c[0].w = sq.x; c[1].w = sq.y; c[2].w = sq.z; c[3].w = sq.w;
+      }
       if (noise != nullptr) nz = *reinterpret_cast<const float4*>(noise + p0);
       if (g_w != nullptr) gwq = *reinterpret_cast<const float4*>(g_w + p0);
       const float dx = rays[ray * 8 + 3], dy = rays[ray * 8 + 4], dz = rays[ray * 8 + 5];
@@ -654,14 +663,17 @@ __global__ void __launch_bounds__(256) composite_bwd4_kernel(
     if (sl == L - 1) tail = 0.f;
     const float suf[4] = {tail + s0, tail + s1, tail + s2, tail};
     if (act) {
+      float gs[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const float w = q.alpha[k] * q.T[k];
         const float galpha = gw[k] * q.T[k] - suf[k] / (__fadd_rn(__fsub_rn(1.0f, q.alpha[k]), 1e-10f));
         const float gsig = q.sg[k] > 0.f ? galpha * q.delta[k] * q.e[k] : 0.f;
-        reinterpret_cast<float4*>(g_raw)[p0 + k] = make_float4(gr * w, gg * w, gb * w, gsig);
+        gs[k] = gsig;
+        if (raw_channels == 4) reinterpret_cast<float4*>(g_raw)[p0 + k] = make_float4(gr * w, gg * w, gb * w, gsig);
         amax = fmaxf(fmaxf(amax, fabsf(gsig)), fmaxf(fmaxf(fabsf(gr * w), fabsf(gg * w)), fabsf(gb * w)));
       }
+      if (raw_channels == 1) *reinterpret_cast<float4*>(g_raw + p0) = make_float4(gs[0], gs[1], gs[2], gs[3]);
     }
   }
   if (g_amax != nullptr) {
@@ -1050,7 +1062,7 @@ int launch_composite(const float* raw, int raw_channels, const float* z, const f
   return check_launch("composite_fwd_kernel");
 }
 
-int launch_composite_bwd(const float* raw, const float* z, const float* rays, const float* noise, float noise_std,
+int launch_composite_bwd(const float* raw, int raw_channels, const float* z, const float* rays, const float* noise, float noise_std,
                           int white_back, const float* g_rgb, const float* g_depth, const float* g_w, int64_t n_rays,
                           int S, float* g_raw, const SnbLossSpec* loss, const float* out_rgb, const float* out_depth,
                           const float* g_loss, float* g_amax, cudaStream_t st) {
@@ -1060,9 +1072,9 @@ int launch_composite_bwd(const float* raw, const float* z, const float* rays, co
     const int grid = grid_for(n_rays, 8 * (32 / L), sm_count() * 6);
     const LossSpec ls = make_loss_spec(loss);
     unsigned int* am = reinterpret_cast<unsigned int*>(g_amax);
-    if (L == 8) composite_bwd4_kernel<8><<<grid, 256, 0, st>>>(raw, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w, n_rays, S, g_raw, ls, out_rgb, out_depth, g_loss, am);
-    else if (L == 16) composite_bwd4_kernel<16><<<grid, 256, 0, st>>>(raw, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w, n_rays, S, g_raw, ls, out_rgb, out_depth, g_loss, am);
-    else composite_bwd4_kernel<32><<<grid, 256, 0, st>>>(raw, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w, n_rays, S, g_raw, ls, out_rgb, out_depth, g_loss, am);
+    if (L == 8) composite_bwd4_kernel<8><<<grid, 256, 0, st>>>(raw, raw_channels, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w, n_rays, S, g_raw, ls, out_rgb, out_depth, g_loss, am);
+    else if (L == 16) composite_bwd4_kernel<16><<<grid, 256, 0, st>>>(raw, raw_channels, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w, n_rays, S, g_raw, ls, out_rgb, out_depth, g_loss, am);
+    else composite_bwd4_kernel<32><<<grid, 256, 0, st>>>(raw, raw_channels, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w, n_rays, S, g_raw, ls, out_rgb, out_depth, g_loss, am);
     return check_launch("composite_bwd4_kernel");
   }
   const size_t smem = (size_t)8 * 3 * S * sizeof(float);
@@ -1071,7 +1083,7 @@ int launch_composite_bwd(const float* raw, const float* z, const float* rays, co
   if (smem > 48 * 1024)
     if (int rc = ensure_smem(composite_bwd_kernel, optin, (int)smem, "composite_bwd")) return rc;
   const int grid = grid_for(n_rays, 8, sm_count() * 8);
-  composite_bwd_kernel<<<grid, 256, smem, st>>>(raw, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w,
+  composite_bwd_kernel<<<grid, 256, smem, st>>>(raw, raw_channels, z, rays, noise, noise_std, white_back, g_rgb, g_depth, g_w,
                                                 n_rays, S, g_raw, make_loss_spec(loss), out_rgb, out_depth, g_loss,
                                                 reinterpret_cast<unsigned int*>(g_amax));
   return check_launch("composite_bwd_kernel");

@@ -226,6 +226,7 @@ int run_wgrad16(const void* dY, int FA, const void* X, int FB, int K, float* dW,
   if (FA == 256 && FB == 64 && !head) return launch_wgrad16<2, 64, false>(a, st);
   if (FA == 128 && FB == 32 && !head) return launch_wgrad16<1, 32, false>(a, st);
   if (FA == 0 && FB == 128 && head) return launch_wgrad16<0, 128, true>(a, st);
+  if (FA == 0 && FB == 256 && head) return launch_wgrad16<0, 256, true>(a, st);    // sigma-only passes: dW_sigma
   return fail(SNB_ERR_INVALID, "run_wgrad16: unsupported shape FA=%d FB=%d head=%d", FA, FB, (int)head);
 }
 

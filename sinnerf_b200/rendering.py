@@ -210,6 +210,102 @@ class _RenderPass(torch.autograd.Function):
         return (None, None, None, None, None, None, None, None, *grads)
 
 
+# the parameter tensors a sigma-only pass reads: xyz_encoding_1..8 and sigma (state-dict indices 0-15, 20, 21)
+_SIGMA_PASS_TENSORS = tuple(range(16)) + (20, 21)
+
+
+class _SigmaPass(torch.autograd.Function):
+    """One sigma-only field pass: layers 1-8 and the sigma head (models/nerf.py:105-136 with sigma_only=True), and with
+    `composite` the weights-only compositing after it (models/rendering.py:215-238 with weights_only=True).
+
+    composite=True returns the weights (N,S): render_rays(test_time=True)'s coarse pass (rendering.py:287-292).
+    composite=False returns sigma (N,S): eval_points (rendering.py:64-123), whose points are staged as rays.
+    Forward: snb_field_forward_train[16]_sigma (+ snb_composite_forward with raw_channels = 1).  Backward:
+    (snb_composite_backward_weights +) snb_field_backward[16]_sigma.  Differentiable in the parameter tensors only;
+    xyz_encoding_final, dir_encoding and rgb, which the pass never reads, get None, as autograd through the reference
+    leaves them."""
+
+    @staticmethod
+    def forward(ctx, model: "NeRF", prec: int, rays, z, noise, noise_std, composite, *params):
+        lib = _lib.load()
+        dev = rays.device
+        n, S = z.shape
+        P = n * S
+        img = model.packed_weights(prec)
+        sigma = torch.empty(n, S, device=dev, dtype=torch.float32)
+        store16 = prec != _lib.PRECISIONS["fp32"] and config.get_train_storage() == "fp16"
+        if store16:
+            act16 = torch.empty(lib.snb_act16_bytes(P), device=dev, dtype=torch.uint8)
+            save_enc = save_h = sigma.new_empty(0)
+        else:
+            act16 = sigma.new_empty(0)
+            save_enc = torch.empty(P, 64, device=dev, dtype=torch.float32)
+            save_h = torch.empty(8, P, 256, device=dev, dtype=torch.float32)
+        w = torch.empty(n, S, device=dev, dtype=torch.float32) if composite else None
+        with torch.cuda.device(dev):
+            st = _lib.stream_ptr(dev)
+            if store16:
+                _lib.check(lib.snb_field_forward_train16_sigma(_lib.ptr(img), prec, _lib.ptr(rays), _lib.ptr(z), n, S,
+                                                               _lib.ptr(sigma), _lib.ptr(act16), st),
+                           "snb_field_forward_train16_sigma")
+            else:
+                _lib.check(lib.snb_field_forward_train_sigma(_lib.ptr(img), prec, _lib.ptr(rays), _lib.ptr(z), n, S,
+                                                             _lib.ptr(sigma), _lib.ptr(save_enc), _lib.ptr(save_h), st),
+                           "snb_field_forward_train_sigma")
+            if composite:
+                _lib.check(lib.snb_composite_forward(_lib.ptr(sigma), 1, _lib.ptr(z), _lib.ptr(rays), _lib.ptr(noise),
+                                                     noise_std, 0, n, S, None, None, _lib.ptr(w), st),
+                           "snb_composite_forward")
+        ctx.save_for_backward(sigma, z, rays, noise if noise is not None else sigma.new_empty(0), save_enc, save_h,
+                              act16, *params)
+        ctx.cfg = (float(noise_std), noise is not None, store16, bool(composite))
+        return w if composite else sigma
+
+    @staticmethod
+    def backward(ctx, g_out):
+        lib = _lib.load()
+        sigma, z, rays, noise, save_enc, save_h, act16, *params = ctx.saved_tensors
+        noise_std, has_noise, store16, composite = ctx.cfg
+        dev = sigma.device
+        n, S = z.shape
+        P = n * S
+        ps = [p.detach().contiguous() for p in params]
+        # one zero-filled buffer for the gradients the pass produces (the kernels accumulate into them)
+        offs, total = {}, 0
+        for i in _SIGMA_PASS_TENSORS:
+            offs[i] = total
+            total += (ps[i].numel() + 3) // 4 * 4
+        flat = torch.zeros(total, device=dev, dtype=torch.float32)
+        grads = [flat[offs[i]:offs[i] + p.numel()].view_as(p) if i in offs else None for i, p in enumerate(ps)]
+        parr = (C.c_void_p * 24)(*[p.data_ptr() for p in ps])
+        garr = (C.c_void_p * 24)(*[g.data_ptr() if g is not None else None for g in grads])
+        g = g_out.contiguous().to(torch.float32)
+        with torch.cuda.device(dev):
+            st = _lib.stream_ptr(dev)
+            g_amax = None
+            if composite:
+                g_amax = torch.zeros(1, device=dev, dtype=torch.float32) if store16 else None   # bit pattern of max |g_sigma|
+                g_sigma = torch.empty_like(sigma)
+                _lib.check(lib.snb_composite_backward_weights(_lib.ptr(sigma), _lib.ptr(z), _lib.ptr(rays),
+                                                              _lib.ptr(noise) if has_noise else None, noise_std,
+                                                              _lib.ptr(g), n, S, _lib.ptr(g_sigma), _lib.ptr(g_amax), st),
+                           "snb_composite_backward_weights")
+            else:
+                g_sigma = g
+            if store16:
+                ws = torch.empty(lib.snb_bwd16_workspace_bytes(P), device=dev, dtype=torch.uint8)
+                _lib.check(lib.snb_field_backward16_sigma(parr, garr, _lib.ptr(g_sigma), _lib.ptr(act16), P, _lib.ptr(ws),
+                                                          _lib.ptr(g_amax), st), "snb_field_backward16_sigma")
+            else:
+                ws_a = torch.empty(P, 256, device=dev, dtype=torch.float32)
+                ws_b = torch.empty(P, 256, device=dev, dtype=torch.float32)
+                ws_m = torch.empty(P, 8, device=dev, dtype=torch.int32)
+                _lib.check(lib.snb_field_backward_sigma(parr, garr, _lib.ptr(g_sigma), _lib.ptr(save_enc), _lib.ptr(save_h),
+                                                        P, _lib.ptr(ws_a), _lib.ptr(ws_b), _lib.ptr(ws_m), st),
+                           "snb_field_backward_sigma")
+        return (None, None, None, None, None, None, None, *grads)
+
+
 class _Composite(torch.autograd.Function):
     """(rgb, depth, weights) = composite(raw, z, ...), backward = snb_composite_backward (closed form).
     Stand-alone differentiable compositing of a given raw tensor (stage tests; the training path uses _RenderPass)."""
@@ -267,16 +363,36 @@ def _field_composite_nograd(model, prec, rays, z, noise, noise_std, white_back):
     return rgb, depth, w
 
 
+def _weights_nograd(model, prec, rays, z, noise, noise_std):
+    """A sigma-only field pass + weights-only compositing with the inference kernels."""
+    lib = _lib.load()
+    dev = rays.device
+    n, S = z.shape
+    sigma = torch.empty(n, S, device=dev, dtype=torch.float32)
+    w = torch.empty(n, S, device=dev, dtype=torch.float32)
+    img = model.packed_weights(prec)
+    with torch.cuda.device(dev):
+        st = _lib.stream_ptr(dev)
+        _lib.check(lib.snb_field_forward(_lib.ptr(img), prec, _lib.ptr(rays), _lib.ptr(z), n, S, 1, _lib.ptr(sigma), st),
+                   "snb_field_forward")
+        _lib.check(lib.snb_composite_forward(_lib.ptr(sigma), 1, _lib.ptr(z), _lib.ptr(rays), _lib.ptr(noise), noise_std,
+                                             0, n, S, None, None, _lib.ptr(w), st), "snb_composite_forward")
+    return w
+
+
 def _needs_grad(models) -> bool:
     return torch.is_grad_enabled() and any(p.requires_grad for m in models for p in m.parameters())
 
 
 def _render_rays_train(models, r, S, Ni, use_disp, perturb, noise_std, white_back, detach_coarse, rng_draw,
-                       return_intermediates=False, prec: int = 0, losses: Optional[RayLosses] = None):
+                       return_intermediates=False, prec: int = 0, losses: Optional[RayLosses] = None,
+                       test_time: bool = False):
     """render_rays with autograd (reference models/rendering.py:126-335 under grad mode): same
     kernels for sampling / importance sampling, the field pass that keeps activations (in the
     arithmetic of `prec`: tensor-core modes or the fp32 FFMA kernel), the closed-form compositing
-    backward and the tensor-core / FFMA MLP backward.  Gradients reach the NeRF parameters only."""
+    backward and the tensor-core / FFMA MLP backward.  Gradients reach the NeRF parameters only.
+    test_time: the coarse pass is sigma-only (rendering.py:287-292) and yields only its weights; the loss terms
+    come from the fine pass alone."""
     lib = _lib.load()
     dev = r.device
     n = r.shape[0]
@@ -307,12 +423,20 @@ def _render_rays_train(models, r, S, Ni, use_disp, perturb, noise_std, white_bac
             loss_terms[which] = loss
         return rgb, depth, w
 
+    def sigma_pass(model, z, noise):
+        nz = noise if noise_std != 0 else None
+        if not (torch.is_grad_enabled() and any(p.requires_grad for p in model.parameters())):
+            return _weights_nograd(model, prec, r, z, nz, noise_std)
+        return _SigmaPass.apply(model, prec, r, z, nz, noise_std, True, *model._param_list())
+
+    coarse_pass = (lambda: (None, None, sigma_pass(models[0], z_c, noise_c))) if test_time else \
+        (lambda: field_pass(models[0], z_c, noise_c, "coarse"))
     if detach_coarse:
         with torch.no_grad():
-            rgb_c, depth_c, w_c = field_pass(models[0], z_c, noise_c, "coarse")
+            rgb_c, depth_c, w_c = coarse_pass()
     else:
-        rgb_c, depth_c, w_c = field_pass(models[0], z_c, noise_c, "coarse")
-    result = {"rgb_coarse": rgb_c, "depth_coarse": depth_c, "opacity_coarse": w_c}
+        rgb_c, depth_c, w_c = coarse_pass()
+    result = {"opacity_coarse": w_c} if test_time else {"rgb_coarse": rgb_c, "depth_coarse": depth_c, "opacity_coarse": w_c}
     if Ni > 0:
         det = not (perturb > 0)
         pdf_u = None if det else rng_draw("pdf_u", torch.rand, n, Ni)
@@ -376,9 +500,30 @@ def sample_pdf(bins, weights, N_importance, det=False, eps=1e-5, *, _u: Optional
 
 
 def eval_points(points, models, embeddings):
-    """sigma of the fine model at 3-D points, reference models/rendering.py:64-123
-    (imported by models/sinnerf.py:13, never called there)."""
-    return models[-1](embeddings[0](points), sigma_only=True)
+    """sigma (B,1) of the fine model at 3-D points (B,3), reference models/rendering.py:64-123
+    (imported by models/sinnerf.py:13, never called there).
+
+    Under autograd (grad mode on and a parameter of the fine model requiring grad) the gradients reach that model's
+    parameters, through the sigma-only training kernels: each point is staged as a ray [x, 0, 0, 0, 0, 0] with one
+    sample at z = 0, so the kernel's o + d z is exactly x.  The points themselves are not differentiated."""
+    model = models[-1]
+    if not _needs_grad([model]):
+        return model(embeddings[0](points), sigma_only=True)
+    _lib.require_device(points, "eval_points")
+    if points.requires_grad:
+        raise NotImplementedError("sinnerf_b200.eval_points is not differentiable in the points (as Embedding.forward); "
+                                  "detach them")
+    emb = embeddings[0]
+    if (emb.N_freqs, emb.in_channels, emb._logscale) != (10, 3, True):
+        raise NotImplementedError("eval_points: the training kernels are built for Embedding(3, 10) (logscale)")
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError(f"eval_points: expected points (B, 3), got {tuple(points.shape)}")
+    n = points.shape[0]
+    rays = torch.zeros(n, 8, device=points.device, dtype=torch.float32)
+    rays[:, :3] = points.detach()
+    z = torch.zeros(n, 1, device=points.device, dtype=torch.float32)
+    prec = _lib.precision_id(config.get_precision())
+    return _SigmaPass.apply(model, prec, rays, z, None, 0.0, False, *model._param_list())
 
 
 def render_rays(models,
@@ -410,7 +555,9 @@ def render_rays(models,
     activation ever reaches HBM in inference, so there is nothing to chunk.  Under autograd (grad
     mode on and a model parameter requiring grad) the call runs the training path: the field
     pass that also keeps activations + hand-written tensor-core backward kernels; gradients reach
-    the NeRF parameters only, as in the reference.  `noisy_coarse` is ignored exactly
+    the NeRF parameters only, as in the reference; with `test_time=True` the coarse pass is the
+    sigma-only one there too (its `opacity_coarse` differentiates into the coarse trunk and sigma
+    head, the loss terms come from the fine pass).  `noisy_coarse` is ignored exactly
     as in the reference (:138).  Keyword-only extras: `precision` overrides
     sinnerf_b200.config; `losses` (a RayLosses, training path only) evaluates the MSE-rgb / SmoothL1-depth
     terms of models/sinnerf.py:310-319 inside the compositing kernels and adds `loss_rgb`, `loss_depth`
@@ -451,11 +598,8 @@ def render_rays(models,
     if _needs_grad(models[:2 if Ni > 0 else 1]):
         if pixel_scatter is not None:
             raise ValueError("render_rays(pixel_scatter=...) is an inference feature: call it under torch.no_grad()")
-        if test_time:
-            raise NotImplementedError("render_rays(test_time=True) under autograd is not built (the reference "
-                                      "never trains with it: models/sinnerf.py:176-186)")
         return _render_rays_train(models, r, S, Ni, bool(use_disp), perturb, noise_std, bool(white_back),
-                                  bool(detach_coarse), rnd, _return_intermediates, prec, losses)
+                                  bool(detach_coarse), rnd, _return_intermediates, prec, losses, bool(test_time))
     if losses is not None:
         raise ValueError("render_rays(losses=...) is the training path: it needs grad mode and trainable NeRF parameters")
     scatter = None
