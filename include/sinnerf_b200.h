@@ -44,11 +44,15 @@ extern "C" {
  *             in registers -- meets the <=1e-4 fp32 parity bar on tensor cores
  *  BF16X3   : same with bf16 halves (wider range, ~2e-5)
  *  BF16     : single-pass bf16 operands, fp32 accumulate (BASELINE.json configs[2])
+ *  F16      : fp16 operands, one product, fp32 accumulate: the reference under `precision=16`
+ *             (Lightning's native AMP: nn.Linear in fp16, everything else fp32); operands
+ *             saturate at +-65504
  */
 #define SNB_PREC_FP32 0
 #define SNB_PREC_F16X3 1
 #define SNB_PREC_BF16X3 2
 #define SNB_PREC_BF16 3
+#define SNB_PREC_F16 4
 
 /* Field MLP shape: NeRF(D=8, W=256, in_channels_xyz=63, in_channels_dir=27, skips=[4])
  * (models/nerf.py:47-50), the only shape SinNeRF instantiates (models/sinnerf.py:137,140).

@@ -16,6 +16,10 @@ LIB_PATH = os.environ.get("SNB_LIB_PATH") or os.path.join(_PKG, "libsinnerf_b200
 
 SNB_OK = 0
 PRECISIONS = {"fp32": 0, "f16x3": 1, "bf16x3": 2, "bf16": 3}
+# Modes kept out of PRECISIONS: the parity tests enumerate that table and hold every mode in it except bf16 / bf16x3 to
+# the fp32 bar (1e-4).  The single-product fp16 mode (SNB_PREC_F16, the reference's arithmetic under Lightning's
+# precision=16) is not fp32-accurate; it has tests of its own against an oracle with the same operand rounding.
+REDUCED_PRECISIONS = {"f16": 4}
 
 c_f = C.c_void_p  # device pointers travel as void*
 
@@ -163,7 +167,7 @@ def stream_ptr(device) -> C.c_void_p:
 def precision_id(name) -> int:
     if isinstance(name, int):
         return name
-    try:
-        return PRECISIONS[name]
-    except KeyError:
-        raise ValueError(f"unknown precision '{name}'; choose one of {sorted(PRECISIONS)}") from None
+    mode = PRECISIONS.get(name, REDUCED_PRECISIONS.get(name))
+    if mode is None:
+        raise ValueError(f"unknown precision '{name}'; choose one of {sorted(PRECISIONS) + sorted(REDUCED_PRECISIONS)}")
+    return mode

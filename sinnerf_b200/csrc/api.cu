@@ -82,7 +82,7 @@ int field_forward_train_tc(const void*, int, const float*, const float*, int64_t
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 static int check_precision(int precision) {
-  if (precision < SNB_PREC_FP32 || precision > SNB_PREC_BF16)
+  if (precision < SNB_PREC_FP32 || precision > SNB_PREC_F16)
     return fail(SNB_ERR_INVALID, "unknown precision mode %d", precision);
   return SNB_OK;
 }
@@ -116,7 +116,7 @@ int snb_device_check(int* sm_count, int* cc_major, int* cc_minor) {
 
 size_t snb_packed_weights_bytes(int precision) {
   if (precision == SNB_PREC_FP32) return sizeof(PackedHeader) + sizeof(float) * (size_t)make_fp32_layout().total;
-  if (precision >= SNB_PREC_F16X3 && precision <= SNB_PREC_BF16) return tc_packed_bytes(precision);
+  if (precision >= SNB_PREC_F16X3 && precision <= SNB_PREC_F16) return tc_packed_bytes(precision);
   return 0;
 }
 

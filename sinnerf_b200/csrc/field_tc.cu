@@ -16,13 +16,13 @@
 //     writes its accumulator without reading it (scale-d = 0).  The epilogue runs in 32-column blocks, each one
 //     K chunk of the next layer's input, interleaved with the wgmmas still in flight (see trunk_layer);
 //   * weights stream from L2 through a shared-memory ring of chunks (128 output rows x 32 K x {hi, lo};
-//     4 stages in the split modes, 18 in bf16) with cp.async.bulk (1-D TMA) + mbarrier complete_tx, issued
-//     by one producer thread that runs ahead over all of the CTA's tiles; the consumers only wait on
+//     4 stages in the split modes, 18 in the single-product modes) with cp.async.bulk (1-D TMA) + mbarrier
+//     complete_tx, issued by one producer thread that runs ahead over all of the CTA's tiles; the consumers only wait on
 //     `full` and release stages.  The packed image is laid out in exactly the order the warpgroups consume
 //     it, in the same canonical layout, so a chunk is one contiguous copy;
 //   * fp32 parity (SNB_PREC_F16X3 / BF16X3): x*w ~= xh*wh + xl*wh + xh*wl, three wgmmas per K step
 //     with fp32 accumulation -- 22 (fp16) or 16 (bf16) significand bits per operand;
-//     SNB_PREC_BF16 is the single product;
+//     SNB_PREC_BF16 and SNB_PREC_F16 are the single product (fp16 operands saturate at +-65504);
 //   * positional encodings (63->64, 27->32 columns) are computed into shared memory in the canonical
 //     layout and consumed at layers 1, 5 (skip) and the direction layer, so neither concat exists; the
 //     xyz encoding is written at the start of a tile, the direction encoding over it once the skip
@@ -199,7 +199,9 @@ __host__ __device__ constexpr bool trunk_biases_strided() {   // the trunk epilo
 static_assert(trunk_biases_strided(), "trunk layer l's bias starts at l * kWidth in the image's constants");
 constexpr size_t kConstBytes = (size_t)kConstFloats * 4;
 
-__host__ __device__ constexpr bool prec_split(int precision) { return precision != SNB_PREC_BF16; }
+__host__ __device__ constexpr bool prec_split(int precision) {
+  return precision != SNB_PREC_BF16 && precision != SNB_PREC_F16;
+}
 // image bytes of one K16 step of a chunk (hi and lo): 128 rows x 16 K x 2 B (x2)
 __host__ __device__ constexpr uint32_t step_image_bytes(int precision) {
   return (uint32_t)(kNh * 16 * 2 * (prec_split(precision) ? 2 : 1));
@@ -321,10 +323,10 @@ __device__ __forceinline__ float softplus_fast(float s) {
   return fmaf(__log2f(1.0f + t), 0.6931471805599453f, fmaxf(s, 0.0f));   // max(s,0) + log1p(t)  (lg2.approx)
 }
 
-// sin / cos for the positional encoding of the single-product bf16 mode: two-constant Cody-Waite reduction to
-// [-pi, pi] and the MUFU approximations (abs error ~1e-6 for |x| up to ~1e4 -- three orders below bf16's 2^-9
-// rounding of the encoded value), ~8 instructions instead of sincosf's ~50; the encoding of a tile sits between two
-// tiles' MMAs.  The fp32-parity modes keep the accurate sincosf.
+// sin / cos for the positional encoding of the single-product modes: two-constant Cody-Waite reduction to
+// [-pi, pi] and the MUFU approximations (abs error ~1e-6 for |x| up to ~1e4 -- three orders below bf16's 2^-9 and
+// two below fp16's 2^-11 rounding of the encoded value), ~8 instructions instead of sincosf's ~50; the encoding of a
+// tile sits between two tiles' MMAs.  The fp32-parity modes keep the accurate sincosf.
 __device__ __forceinline__ void sincos_fast(float x, float* sn, float* cs) {
   const float k = rintf(x * 0.15915494309189535f);
   float r = fmaf(k, -6.2831854820251465f, x);
@@ -405,6 +407,7 @@ __global__ void pack_tc_kernel(ParamPtrs pp, int precision, int new_activation, 
       *reinterpret_cast<uint16_t*>(base + off) = hi;
       *reinterpret_cast<uint16_t*>(base + part + off) = lo;
     } else {
+      if (!kBf16) w = fminf(fmaxf(w, -65504.f), 65504.f);   // fp16 saturates instead of overflowing, as in split16
       *reinterpret_cast<uint16_t*>(base + off) = cvt16<kBf16>(w);
     }
   }
@@ -415,14 +418,15 @@ int launch_pack_tc(const float* const* params, int precision, int new_activation
   ParamPtrs pp;
   for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) pp.p[i] = params[i];
   unsigned char* img = reinterpret_cast<unsigned char*>(image);
-  if (precision < SNB_PREC_F16X3 || precision > SNB_PREC_BF16)
+  if (precision < SNB_PREC_F16X3 || precision > SNB_PREC_F16)
     return fail(SNB_ERR_INVALID, "launch_pack_tc: precision %d is not a tensor-core mode", precision);
   float* fused = reinterpret_cast<float*>(img + sizeof(PackedHeader) + kConstBytes + chunks_bytes(precision));
   fuse_bottleneck_kernel<<<132, 256, 0, st>>>(pp, fused, reinterpret_cast<const PackedHeader*>(img), only_if_dirty);
   if (int rc = check_launch("fuse_bottleneck_kernel")) return rc;
   if (precision == SNB_PREC_F16X3) pack_tc_kernel<false, true><<<264, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
   else if (precision == SNB_PREC_BF16X3) pack_tc_kernel<true, true><<<264, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
-  else pack_tc_kernel<true, false><<<264, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
+  else if (precision == SNB_PREC_BF16) pack_tc_kernel<true, false><<<264, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
+  else pack_tc_kernel<false, false><<<264, 256, 0, st>>>(pp, precision, new_activation, img, only_if_dirty);
   return check_launch("pack_tc_kernel");
 }
 
@@ -982,6 +986,7 @@ static int dispatch_tc(int precision, const TcParams& p, cudaStream_t st) {
     case SNB_PREC_F16X3: return launch_tc<false, true, kEmbedded, kTrain>(p, st);
     case SNB_PREC_BF16X3: return launch_tc<true, true, kEmbedded, kTrain>(p, st);
     case SNB_PREC_BF16: return launch_tc<true, false, kEmbedded, kTrain>(p, st);
+    case SNB_PREC_F16: return launch_tc<false, false, kEmbedded, kTrain>(p, st);
   }
   return fail(SNB_ERR_INVALID, "precision %d is not a tensor-core mode", precision);
 }

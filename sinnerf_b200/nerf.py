@@ -91,6 +91,7 @@ class NeRF(nn.Module):
         self._packed = {}  # (precision id, device) -> uint8 device tensor
         self._fast = {}    # precision id -> validated pointer table of packed_weights()
         self._last_stream = {}   # precision id -> the stream the image was last refreshed / read on
+        self._last_prec = None   # precision id of the last pass (the image a fused optimiser re-packs under 'autocast')
 
     # ------------------------------------------------------------------ kernels' weight image
     def _check_shape(self):
@@ -128,7 +129,8 @@ class NeRF(nn.Module):
         0.9 ms in all).  The validated pointer table is therefore cached and reused for as long as the 24 storage
         addresses are the ones it was built from (a dtype / device / layout change re-allocates and is re-validated):
         ~10 us per call instead of ~70."""
-        prec = _lib.precision_id(config.get_precision() if precision is None else precision)
+        prec = config.resolve_precision(precision)
+        self._last_prec = prec
         ps = self._param_list()
         ptrs = [p.data_ptr() for p in ps]
         fast = self._fast.get(prec)
@@ -208,7 +210,7 @@ class NeRF(nn.Module):
         need = self.in_channels_xyz if sigma_only else self.in_channels_xyz + self.in_channels_dir
         if x.dim() != 2 or x.shape[1] != need:
             raise ValueError(f"NeRF.forward: expected (B, {need}), got {tuple(x.shape)}")
-        prec = _lib.precision_id(config.get_precision())
+        prec = config.resolve_precision()
         image = self.packed_weights(prec)
         xc = x.detach().to(torch.float32).contiguous()
         out = torch.empty(xc.shape[0], 1 if sigma_only else 4, device=x.device, dtype=torch.float32)

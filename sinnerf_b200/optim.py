@@ -81,8 +81,8 @@ class FusedAdam(torch.optim.Optimizer):
         self._steps += 1
         args = _lib.SnbAdamArgs(float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]),
                                 float(g["weight_decay"]), self._steps)
-        prec = _lib.precision_id(config.get_precision() if self._precision is None else self._precision)
         for m, (ea, es) in zip(self.models, self._flat):
+            prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
             ps = m._param_list()
             dev = ps[0].device
             for p in ps:
@@ -178,8 +178,8 @@ class _FusedPerTensor(torch.optim.Optimizer):
         group = self.param_groups[0]
         args = self._args(group)
         adv = self._advances(group)
-        prec = _lib.precision_id(config.get_precision() if self._precision is None else self._precision)
         for m, bufs in zip(self.models, self._flat):
+            prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
             ps = m._param_list()
             dev = ps[0].device
             for p in ps:

@@ -522,7 +522,7 @@ def eval_points(points, models, embeddings):
     rays = torch.zeros(n, 8, device=points.device, dtype=torch.float32)
     rays[:, :3] = points.detach()
     z = torch.zeros(n, 1, device=points.device, dtype=torch.float32)
-    prec = _lib.precision_id(config.get_precision())
+    prec = config.resolve_precision()
     return _SigmaPass.apply(model, prec, rays, z, None, 0.0, False, *model._param_list())
 
 
@@ -559,7 +559,7 @@ def render_rays(models,
     sigma-only one there too (its `opacity_coarse` differentiates into the coarse trunk and sigma
     head, the loss terms come from the fine pass).  `noisy_coarse` is ignored exactly
     as in the reference (:138).  Keyword-only extras: `precision` overrides
-    sinnerf_b200.config; `losses` (a RayLosses, training path only) evaluates the MSE-rgb / SmoothL1-depth
+    sinnerf_b200.config (a mode name, or 'autocast': the mode follows CUDA autocast); `losses` (a RayLosses, training path only) evaluates the MSE-rgb / SmoothL1-depth
     terms of models/sinnerf.py:310-319 inside the compositing kernels and adds `loss_rgb`, `loss_depth`
     (0-dim, differentiable; coarse + fine) and `loss_coarse` / `loss_fine` ((2,) each) to the result;
     `pixel_scatter` (inference only; `(destination addresses, row offset)`, see distributed.PeerPixels) makes the last
@@ -579,7 +579,7 @@ def render_rays(models,
     if test_time and Ni == 0:
         # the reference fails at models/rendering.py:331 (rgb_coarse is never bound)
         raise UnboundLocalError("render_rays(test_time=True) requires N_importance > 0, as in the reference")
-    prec = _lib.precision_id(config.get_precision() if precision is None else precision)
+    prec = config.resolve_precision(precision)
     rng = dict(_rng or {})
     perturb = float(perturb)
     noise_std = float(noise_std)
