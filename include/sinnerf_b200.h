@@ -275,6 +275,47 @@ int snb_field_backward16_sigma(const float* const* params, float* const* grads, 
                                const void* act16, int64_t n_points, void* workspace, const float* g_amax,
                                void* stream);
 
+/* ---- image-space patch losses on render_rays' outputs ------------------------------------------------
+ * The two kornia 0.6.3 losses the training step puts on (B,C,H,W) patches of rendered pixels:
+ *   inverse_depth_smoothness_loss  models/sinnerf.py:370-373, :395-398 (kornia.losses, imported at :23)
+ *   ssim_loss, window_size 11      losses.py:105 (kornia.losses, imported at :2)
+ * Every tensor argument comes with `*_strides`: a HOST array of four int64 ELEMENT strides (N, C, H, W), so
+ * permuted views such as '(b p q) c -> b c p q' of a ray-major (N,3) output are read in place, and gradients are
+ * written with whatever strides the caller chose.  Losses are fp32 scalars; their means use the deterministic
+ * reduction of snb_composite_forward_loss on the same zero-initialised SNB_LOSS_WS_FLOATS scratch.  The backwards
+ * read the upstream gradient g_loss (device, one float) on the device and use no atomics: the result is the same
+ * bits on every run, and scaling g_loss scales every gradient exactly. */
+
+/* inverse_depth_smoothness_loss(idepth (B,1,H,W), image (B,C,H,W)), H, W >= 2:
+ *   mean |dx(idepth) exp(-mean_c |dx(image)|)| + mean |dy(idepth) exp(-mean_c |dy(image)|)|,
+ *   dx(t) = t[..., :, :-1] - t[..., :, 1:], dy likewise along H.  -> loss (1 float) */
+int snb_depth_smooth_forward(const float* idepth, const int64_t* idepth_strides, const float* image,
+                             const int64_t* image_strides, int64_t batch, int channels, int height, int width,
+                             float* loss, float* loss_ws, void* stream);
+/* Its backward: g_idepth (B,1,H,W) and g_image (B,C,H,W) = g_loss * dloss/d(input); either may be NULL (not formed,
+ * its strides may then be NULL too).  |.| differentiates as torch.abs, with sign(0) = 0. */
+int snb_depth_smooth_backward(const float* idepth, const int64_t* idepth_strides, const float* image,
+                              const int64_t* image_strides, int64_t batch, int channels, int height, int width,
+                              const float* g_loss, float* g_idepth, const int64_t* g_idepth_strides, float* g_image,
+                              const int64_t* g_image_strides, void* stream);
+
+/* ssim_loss(img1, img2, window_size, max_val, eps, reduction='mean') on (B,C,H,W) images, H, W >= 6: reflect padding
+ * of 5, depthwise correlation with the 11x11 Gaussian window (sigma 1.5) of img1, img2, img1^2, img2^2, img1 img2, and
+ * mean clamp((1 - ssim) / 2, 0, 1), C1 = (0.01 max_val)^2, C2 = (0.03 max_val)^2.  window_size other than 11:
+ * SNB_ERR_UNSUPPORTED.  The window sums and the SSIM expression are evaluated in fp64 (see DESIGN.md section 4).
+ * coef: NULL (no backward), or a device buffer of 3 B C H W doubles the forward fills with the per-pixel
+ * coefficient maps snb_ssim_loss_backward reads.  -> loss (1 float) */
+int snb_ssim_loss_forward(const float* img1, const int64_t* img1_strides, const float* img2,
+                          const int64_t* img2_strides, int64_t batch, int channels, int height, int width,
+                          int window_size, float max_val, float eps, float* loss, double* coef, float* loss_ws,
+                          void* stream);
+/* Its backward with respect to img1 only (the reference's img2 is always a target):
+ * g_img1 (B,C,H,W) = g_loss * dloss/dimg1, from the coef maps of the forward on the same img1, img2. */
+int snb_ssim_loss_backward(const float* img1, const int64_t* img1_strides, const float* img2,
+                           const int64_t* img2_strides, int64_t batch, int channels, int height, int width,
+                           const double* coef, const float* g_loss, float* g_img1, const int64_t* g_img1_strides,
+                           void* stream);
+
 /* ---- optimiser step (SURVEY.md 8f-4) --------------------------------------------------------------
  * torch.optim.Adam as the reference configures it (utils/__init__.py:19-21: lr, eps = 1e-8, weight_decay;
  * betas default (0.9, 0.999), amsgrad off), fused over the 24 parameter tensors of one NeRF, followed on the

@@ -112,6 +112,15 @@ SIGNATURES = {
                                            c_f, c_f, c_f, c_f]),
     "snb_field_backward16_sigma": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, C.c_int64, c_f,
                                              c_f, c_f]),
+    "snb_depth_smooth_forward": (C.c_int, [c_f, C.POINTER(C.c_int64), c_f, C.POINTER(C.c_int64), C.c_int64, C.c_int,
+                                           C.c_int, C.c_int, c_f, c_f, c_f]),
+    "snb_depth_smooth_backward": (C.c_int, [c_f, C.POINTER(C.c_int64), c_f, C.POINTER(C.c_int64), C.c_int64, C.c_int,
+                                            C.c_int, C.c_int, c_f, c_f, C.POINTER(C.c_int64), c_f, C.POINTER(C.c_int64),
+                                            c_f]),
+    "snb_ssim_loss_forward": (C.c_int, [c_f, C.POINTER(C.c_int64), c_f, C.POINTER(C.c_int64), C.c_int64, C.c_int,
+                                        C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, c_f, c_f, c_f, c_f]),
+    "snb_ssim_loss_backward": (C.c_int, [c_f, C.POINTER(C.c_int64), c_f, C.POINTER(C.c_int64), C.c_int64, C.c_int,
+                                         C.c_int, C.c_int, c_f, c_f, c_f, C.POINTER(C.c_int64), c_f]),
 }
 BWD_WS_FLOATS = 2 * 128 * 256 + 128   # SNB_BWD_WS_FLOATS
 

@@ -79,7 +79,31 @@ int mlp_forward_tc(const void*, int, const float*, int64_t, int64_t, int, float*
 int field_forward_train_tc(const void*, int, const float*, const float*, int64_t, int, int, float*, float*, float*, float*,
                            float*, cudaStream_t);
 
+// image-space patch losses (patch_loss.cu)
+int launch_depth_smooth_fwd(const float*, const int64_t*, const float*, const int64_t*, long long, int, int, int, float*,
+                            float*, cudaStream_t);
+int launch_depth_smooth_bwd(const float*, const int64_t*, const float*, const int64_t*, long long, int, int, int,
+                            const float*, float*, const int64_t*, float*, const int64_t*, cudaStream_t);
+int launch_ssim_fwd(const float*, const int64_t*, const float*, const int64_t*, long long, int, int, int, float, float,
+                    float*, double*, float*, cudaStream_t);
+int launch_ssim_bwd(const float*, const int64_t*, const float*, const int64_t*, long long, int, int, int, const double*,
+                    const float*, float*, const int64_t*, cudaStream_t);
+
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// a (B,C,H,W) patch-loss operand: data and its four element strides, both non-null, strides non-negative
+static int check_nchw(const char* who, const char* name, const void* data, const int64_t* strides) {
+  SNB_REQUIRE(data != nullptr && strides != nullptr, "%s: null pointer (%s or its strides)", who, name);
+  for (int k = 0; k < 4; ++k) SNB_REQUIRE(strides[k] >= 0, "%s: negative stride in %s", who, name);
+  return SNB_OK;
+}
+
+static int check_patch_extents(const char* who, int64_t batch, int channels, int height, int width, int min_hw) {
+  SNB_REQUIRE(batch >= 1 && channels >= 1, "%s: needs batch >= 1 and channels >= 1 (got %lld, %d)", who,
+              (long long)batch, channels);
+  SNB_REQUIRE(height >= min_hw && width >= min_hw, "%s: needs H, W >= %d (got %d x %d)", who, min_hw, height, width);
+  return SNB_OK;
+}
 
 static int check_precision(int precision) {
   if (precision < SNB_PREC_FP32 || precision > SNB_PREC_F16)
@@ -468,6 +492,64 @@ int snb_optim_step(float* const* params, const float* const* grads, float* exp_a
     if (int rc = check_precision(precision)) return rc;
   return optim_step_pack(params, grads, exp_avg, exp_avg_sq, slow_buffer, *args, precision, new_activation, packed,
                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_depth_smooth_forward(const float* idepth, const int64_t* idepth_strides, const float* image,
+                             const int64_t* image_strides, int64_t batch, int channels, int height, int width,
+                             float* loss, float* loss_ws, void* stream) {
+  const char* who = "snb_depth_smooth_forward";
+  if (int rc = check_patch_extents(who, batch, channels, height, width, 2)) return rc;
+  if (int rc = check_nchw(who, "idepth", idepth, idepth_strides)) return rc;
+  if (int rc = check_nchw(who, "image", image, image_strides)) return rc;
+  SNB_REQUIRE(loss != nullptr && loss_ws != nullptr, "%s: null loss output / workspace", who);
+  return launch_depth_smooth_fwd(idepth, idepth_strides, image, image_strides, batch, channels, height, width, loss,
+                                 loss_ws, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_depth_smooth_backward(const float* idepth, const int64_t* idepth_strides, const float* image,
+                              const int64_t* image_strides, int64_t batch, int channels, int height, int width,
+                              const float* g_loss, float* g_idepth, const int64_t* g_idepth_strides, float* g_image,
+                              const int64_t* g_image_strides, void* stream) {
+  const char* who = "snb_depth_smooth_backward";
+  if (int rc = check_patch_extents(who, batch, channels, height, width, 2)) return rc;
+  if (int rc = check_nchw(who, "idepth", idepth, idepth_strides)) return rc;
+  if (int rc = check_nchw(who, "image", image, image_strides)) return rc;
+  SNB_REQUIRE(g_loss != nullptr, "%s: null pointer (g_loss)", who);
+  if (g_idepth != nullptr)
+    if (int rc = check_nchw(who, "g_idepth", g_idepth, g_idepth_strides)) return rc;
+  if (g_image != nullptr)
+    if (int rc = check_nchw(who, "g_image", g_image, g_image_strides)) return rc;
+  return launch_depth_smooth_bwd(idepth, idepth_strides, image, image_strides, batch, channels, height, width, g_loss,
+                                 g_idepth, g_idepth_strides, g_image, g_image_strides,
+                                 reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_ssim_loss_forward(const float* img1, const int64_t* img1_strides, const float* img2,
+                          const int64_t* img2_strides, int64_t batch, int channels, int height, int width,
+                          int window_size, float max_val, float eps, float* loss, double* coef, float* loss_ws,
+                          void* stream) {
+  const char* who = "snb_ssim_loss_forward";
+  if (window_size != 11) return fail(SNB_ERR_UNSUPPORTED, "%s: only window_size 11 is built (got %d)", who, window_size);
+  if (int rc = check_patch_extents(who, batch, channels, height, width, 6)) return rc;
+  if (int rc = check_nchw(who, "img1", img1, img1_strides)) return rc;
+  if (int rc = check_nchw(who, "img2", img2, img2_strides)) return rc;
+  SNB_REQUIRE(loss != nullptr && loss_ws != nullptr, "%s: null loss output / workspace", who);
+  return launch_ssim_fwd(img1, img1_strides, img2, img2_strides, batch, channels, height, width, max_val, eps, loss,
+                         coef, loss_ws, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_ssim_loss_backward(const float* img1, const int64_t* img1_strides, const float* img2,
+                           const int64_t* img2_strides, int64_t batch, int channels, int height, int width,
+                           const double* coef, const float* g_loss, float* g_img1, const int64_t* g_img1_strides,
+                           void* stream) {
+  const char* who = "snb_ssim_loss_backward";
+  if (int rc = check_patch_extents(who, batch, channels, height, width, 6)) return rc;
+  if (int rc = check_nchw(who, "img1", img1, img1_strides)) return rc;
+  if (int rc = check_nchw(who, "img2", img2, img2_strides)) return rc;
+  if (int rc = check_nchw(who, "g_img1", g_img1, g_img1_strides)) return rc;
+  SNB_REQUIRE(coef != nullptr && g_loss != nullptr, "%s: null pointer (coef or g_loss)", who);
+  return launch_ssim_bwd(img1, img1_strides, img2, img2_strides, batch, channels, height, width, coef, g_loss, g_img1,
+                         g_img1_strides, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_render_forward(const SnbRenderArgs* a, void* stream) {
