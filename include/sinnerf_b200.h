@@ -316,6 +316,29 @@ int snb_ssim_loss_backward(const float* img1, const int64_t* img1_strides, const
                            const double* coef, const float* g_loss, float* g_img1, const int64_t* g_img1_strides,
                            void* stream);
 
+/* ---- forward warp: the datasets' depth-warped pseudo-view labels --------------------------------------
+ * The reference view splatted into P source views through its depth, as the datasets build their geometry
+ * pseudo-labels:
+ *   SNB_WARP_ZBUFFER  painter's algorithm, nearest depth wins: datasets/llff_ray_patch_1image_proj.py:144-166,
+ *                     datasets/dtu_proj.py:236-273
+ *   SNB_WARP_LAST     numpy scatter, the last source in raster order wins: datasets/blender_ray_patch_1image_rot3d.py
+ *                     :130-150, datasets/blender_ray_patch_1image_proj.py:120-138 (whose depth_mask is `hit`)
+ * image (H,W,3) and depth (H,W): the reference view, fp32.  mats: P row-major 3x4 fp64 matrices, the top three rows of
+ * src_proj @ inv(ref_proj) (sinnerf_b200.warp composes them as I + (src_proj - ref_proj) inv(ref_proj)) for full
+ * 4x4 projections [[K,0],[0,1]] @ E.  Source pixel (r, c) with d = depth[r,c] goes
+ * to X = ((M00 (c d) + M01 (r d)) + M02 d) + M03 (Y, Z alike), every product and sum rounded on its own (no FMA),
+ * x' = X / Z, y' = Y / Z in fp64 (divided by 1e-9 where Z == 0); target (clamp(floor(y'), 0, H-1), clamp(floor(x'), 0, W-1)),
+ * depth zf = (float)Z.  A source with a non-finite d or a NaN coordinate is skipped.  The occlusion rule and why it
+ * equals the painter loop: DESIGN.md section 4.4.  Outputs (P,H,W,3) rgb, (P,H,W) depth, (P,H,W) hit (bytes 0 / 1);
+ * a pixel nothing landed on is 0.  The result is the same bits on every run.  H*W < 2^31.  workspace: a device
+ * buffer of snb_forward_warp_workspace_bytes(P, H, W, occlusion) bytes, any content (the call initialises it). */
+#define SNB_WARP_ZBUFFER 0
+#define SNB_WARP_LAST 1
+size_t snb_forward_warp_workspace_bytes(int64_t n_poses, int height, int width, int occlusion);
+int snb_forward_warp(const float* image, const float* depth, int height, int width, const double* mats,
+                     int64_t n_poses, int occlusion, float* out_rgb, float* out_depth, uint8_t* out_hit,
+                     void* workspace, void* stream);
+
 /* ---- optimiser step (SURVEY.md 8f-4) --------------------------------------------------------------
  * torch.optim.Adam as the reference configures it (utils/__init__.py:19-21: lr, eps = 1e-8, weight_decay;
  * betas default (0.9, 0.999), amsgrad off), fused over the 24 parameter tensors of one NeRF, followed on the

@@ -16,4 +16,7 @@ def __getattr__(name):
     if name in ("FusedAdam", "FusedSGD", "FusedRAdam", "FusedRanger", "get_optimizer"):
         from . import optim
         return getattr(optim, name)
+    if name == "forward_warp":
+        from . import warp
+        return warp.forward_warp
     raise AttributeError(name)

@@ -121,7 +121,10 @@ SIGNATURES = {
                                         C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, c_f, c_f, c_f, c_f]),
     "snb_ssim_loss_backward": (C.c_int, [c_f, C.POINTER(C.c_int64), c_f, C.POINTER(C.c_int64), C.c_int64, C.c_int,
                                          C.c_int, C.c_int, c_f, c_f, c_f, C.POINTER(C.c_int64), c_f]),
+    "snb_forward_warp_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int, C.c_int]),
+    "snb_forward_warp": (C.c_int, [c_f, c_f, C.c_int, C.c_int, c_f, C.c_int64, C.c_int, c_f, c_f, c_f, c_f, c_f]),
 }
+WARP_OCCLUSION = {"zbuffer": 0, "last": 1}   # SNB_WARP_*
 BWD_WS_FLOATS = 2 * 128 * 256 + 128   # SNB_BWD_WS_FLOATS
 
 _lib = None

@@ -89,6 +89,11 @@ int launch_ssim_fwd(const float*, const int64_t*, const float*, const int64_t*, 
 int launch_ssim_bwd(const float*, const int64_t*, const float*, const int64_t*, long long, int, int, int, const double*,
                     const float*, float*, const int64_t*, cudaStream_t);
 
+// forward warp (warp.cu)
+size_t forward_warp_workspace_bytes(long long, long long, int);
+int launch_forward_warp(const float*, const float*, int, int, const double*, long long, int, float*, float*,
+                        unsigned char*, void*, cudaStream_t);
+
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // a (B,C,H,W) patch-loss operand: data and its four element strides, both non-null, strides non-negative
@@ -550,6 +555,32 @@ int snb_ssim_loss_backward(const float* img1, const int64_t* img1_strides, const
   SNB_REQUIRE(coef != nullptr && g_loss != nullptr, "%s: null pointer (coef or g_loss)", who);
   return launch_ssim_bwd(img1, img1_strides, img2, img2_strides, batch, channels, height, width, coef, g_loss, g_img1,
                          g_img1_strides, reinterpret_cast<cudaStream_t>(stream));
+}
+
+static int check_warp_extents(const char* who, int64_t n_poses, int height, int width, int occlusion) {
+  SNB_REQUIRE(occlusion == SNB_WARP_ZBUFFER || occlusion == SNB_WARP_LAST, "%s: unknown occlusion mode %d", who,
+              occlusion);
+  SNB_REQUIRE(n_poses >= 1, "%s: needs n_poses >= 1 (got %lld)", who, (long long)n_poses);
+  SNB_REQUIRE(height >= 1 && width >= 1 && (int64_t)height * width < (int64_t(1) << 31),
+              "%s: needs H, W >= 1 and H*W < 2^31 (got %d x %d)", who, height, width);
+  return SNB_OK;
+}
+
+size_t snb_forward_warp_workspace_bytes(int64_t n_poses, int height, int width, int occlusion) {
+  if (check_warp_extents("snb_forward_warp_workspace_bytes", n_poses, height, width, occlusion)) return 0;
+  return forward_warp_workspace_bytes(n_poses, (long long)height * width, occlusion);
+}
+
+int snb_forward_warp(const float* image, const float* depth, int height, int width, const double* mats,
+                     int64_t n_poses, int occlusion, float* out_rgb, float* out_depth, uint8_t* out_hit,
+                     void* workspace, void* stream) {
+  const char* who = "snb_forward_warp";
+  if (int rc = check_warp_extents(who, n_poses, height, width, occlusion)) return rc;
+  SNB_REQUIRE(image != nullptr && depth != nullptr && mats != nullptr, "%s: null pointer (image, depth or mats)", who);
+  SNB_REQUIRE(out_rgb != nullptr && out_depth != nullptr && out_hit != nullptr && workspace != nullptr,
+              "%s: null pointer (an output or the workspace)", who);
+  return launch_forward_warp(image, depth, height, width, mats, n_poses, occlusion, out_rgb, out_depth, out_hit,
+                             workspace, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_render_forward(const SnbRenderArgs* a, void* stream) {
