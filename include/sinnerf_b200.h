@@ -339,6 +339,36 @@ int snb_forward_warp(const float* image, const float* depth, int height, int wid
                      int64_t n_poses, int occlusion, float* out_rgb, float* out_depth, uint8_t* out_hit,
                      void* workspace, void* stream);
 
+/* ---- semantic loss: DINO ViT-S/16 CLS feature -------------------------------------------------------
+ * models/sinnerf.py:162-169 get_vit_feature(x): F.interpolate(x, (224, 224)) (nearest), (x - mean) / std with the
+ * ImageNet constants, DINO vit_small/16 (12 pre-norm blocks, width 384, 6 heads of 64, MLP 1536 with exact GELU,
+ * LayerNorm eps 1e-6), and the output of block 11 (before the final norm) at token 0 of image 0.
+ * params: HOST array of SNB_VIT_N_TENSORS device pointers to the fp32 tensors of DINO's state dict in its order,
+ * without the final norm: cls_token, pos_embed, patch_embed.proj.{weight,bias}, then for each of the 12 blocks
+ * norm1.{weight,bias}, attn.qkv.{weight,bias}, attn.proj.{weight,bias}, norm2.{weight,bias}, mlp.fc1.{weight,bias},
+ * mlp.fc2.{weight,bias}.  snb_vit_pack copies them into `image` (snb_vit_pack_bytes(precision) bytes): fp32 vectors
+ * and the GEMM weights as fp16 hi + lo planes (SNB_PREC_FP32, _F16X3, _BF16X3: three products per GEMM) or one
+ * fp16 (SNB_PREC_F16) or bf16 (SNB_PREC_BF16) plane.  Forward and backward must be called with the precision the
+ * image was packed in.  Every GEMM runs on wgmma; LayerNorm, softmax, GELU and the residual stream are fp32. */
+#define SNB_VIT_N_TENSORS 148
+#define SNB_VIT_DIM 384
+#define SNB_VIT_MAX_IMAGES 8
+size_t snb_vit_pack_bytes(int precision);
+int snb_vit_pack(const float* const* params, int precision, void* image, void* stream);
+/* device workspace of a pass over n_images images; save = 1 keeps what snb_vit_backward reads */
+size_t snb_vit_workspace_bytes(int n_images, int save);
+/* CLS features of n_images (1..SNB_VIT_MAX_IMAGES) images in one batched pass.  images: HOST array of device
+ * pointers to (3, h, w) fp32 images read through element strides (HOST, n x 3: channel, row, column); sizes: HOST,
+ * n x 2 (h, w), each >= 1.  -> out (n, 384), row-major.  save = 1: the workspace keeps the activations of the
+ * backward and must be handed to it unchanged. */
+int snb_vit_forward(const void* image, int precision, const float* const* images, const int64_t* strides,
+                    const int* sizes, int n_images, int save, float* out, void* workspace, void* stream);
+/* Gradient of the n features with respect to the n images of the save = 1 forward whose workspace this is:
+ * d_out (n, 384) -> d_images[i] (3, h_i, w_i) written through d_strides (HOST, n x 3).  Every element of each
+ * d_images[i] is written; nothing is accumulated. */
+int snb_vit_backward(const void* image, int precision, const int* sizes, int n_images, const float* d_out,
+                     float* const* d_images, const int64_t* d_strides, void* workspace, void* stream);
+
 /* ---- optimiser step (SURVEY.md 8f-4) --------------------------------------------------------------
  * torch.optim.Adam as the reference configures it (utils/__init__.py:19-21: lr, eps = 1e-8, weight_decay;
  * betas default (0.9, 0.999), amsgrad off), fused over the 24 parameter tensors of one NeRF, followed on the

@@ -123,7 +123,16 @@ SIGNATURES = {
                                          C.c_int, C.c_int, c_f, c_f, c_f, C.POINTER(C.c_int64), c_f]),
     "snb_forward_warp_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int, C.c_int]),
     "snb_forward_warp": (C.c_int, [c_f, c_f, C.c_int, C.c_int, c_f, C.c_int64, C.c_int, c_f, c_f, c_f, c_f, c_f]),
+    "snb_vit_pack_bytes": (C.c_size_t, [C.c_int]),
+    "snb_vit_pack": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, c_f, c_f]),
+    "snb_vit_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "snb_vit_forward": (C.c_int, [c_f, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int),
+                                  C.c_int, C.c_int, c_f, c_f, c_f]),
+    "snb_vit_backward": (C.c_int, [c_f, C.c_int, C.POINTER(C.c_int), C.c_int, c_f, C.POINTER(C.c_void_p),
+                                   C.POINTER(C.c_int64), c_f, c_f]),
 }
+VIT_N_TENSORS = 148       # SNB_VIT_N_TENSORS
+VIT_MAX_IMAGES = 8        # SNB_VIT_MAX_IMAGES
 WARP_OCCLUSION = {"zbuffer": 0, "last": 1}   # SNB_WARP_*
 BWD_WS_FLOATS = 2 * 128 * 256 + 128   # SNB_BWD_WS_FLOATS
 

@@ -110,3 +110,36 @@ def default_init_params(seed: int) -> Dict[str, torch.Tensor]:
     sd = {k: v.detach().clone() for k, v in NeRF(use_new_activation=True).state_dict().items()}
     torch.random.set_rng_state(state)
     return sd
+
+
+def dino_vits16_state_dict(seed: int = 0) -> Dict[str, torch.Tensor]:
+    """Seeded stand-in for DINO ViT-S/16's weights (the released file is not in the repository), with the keys and
+    shapes of dino_deitsmall16_pretrain.pth.  LayerNorm gains and biases and every Linear bias are non-trivial, and the
+    qkv weights (N(0, (1.5/sqrt(384))^2)) give attention logits with a per-layer standard deviation of a few units, so
+    softmax is neither uniform nor one-hot.  Much larger qkv weights make the 12-block stack chaotic: rounding the
+    operands to bf16 alone then moves the CLS feature by tens of percent.  The global RNG state is untouched."""
+    g = torch.Generator().manual_seed(seed)
+
+    def n(*shape, std=1.0):
+        return torch.randn(*shape, generator=g) * std
+
+    d, m = 384, 1536
+    sd = {"cls_token": n(1, 1, d, std=0.5), "pos_embed": n(1, 197, d, std=0.5),
+          "patch_embed.proj.weight": n(d, 3, 16, 16, std=1.0 / math.sqrt(768)), "patch_embed.proj.bias": n(d, std=0.1)}
+    for b in range(12):
+        p = f"blocks.{b}."
+        sd[p + "norm1.weight"] = 1.0 + n(d, std=0.2)
+        sd[p + "norm1.bias"] = n(d, std=0.1)
+        sd[p + "attn.qkv.weight"] = n(3 * d, d, std=1.5 / math.sqrt(d))
+        sd[p + "attn.qkv.bias"] = n(3 * d, std=0.1)
+        sd[p + "attn.proj.weight"] = n(d, d, std=0.5 / math.sqrt(d))
+        sd[p + "attn.proj.bias"] = n(d, std=0.05)
+        sd[p + "norm2.weight"] = 1.0 + n(d, std=0.2)
+        sd[p + "norm2.bias"] = n(d, std=0.1)
+        sd[p + "mlp.fc1.weight"] = n(m, d, std=1.0 / math.sqrt(d))
+        sd[p + "mlp.fc1.bias"] = n(m, std=0.1)
+        sd[p + "mlp.fc2.weight"] = n(d, m, std=0.5 / math.sqrt(m))
+        sd[p + "mlp.fc2.bias"] = n(d, std=0.05)
+    sd["norm.weight"] = 1.0 + n(d, std=0.2)
+    sd["norm.bias"] = n(d, std=0.1)
+    return sd
