@@ -550,7 +550,9 @@ __global__ void vit_fold_kernel(const float* __restrict__ dcol, const float* __r
   *out = acc / kStd[ch] * inv_scale[i];
 }
 
-// per image: s = 2^k with max |g| s in [1, 2) (1 for an all-zero or non-finite row); dx = g s, inv = 1 / s
+// per image: k with max |g| 2^k in [1, 2) (0 for an all-zero or non-finite row); dx = g 2^k, inv = 2^-k.  Both go
+// through ldexpf, never through s = 2^k as a float: for a subnormal max |g|, k reaches 149 and 2^k overflows (inf,
+// then inv = 0 and NaN gradients in the bf16 mode), while g 2^k < 2 and 2^-k >= 2^-149 are exact.
 __global__ void vit_grad_scale_kernel(const float* __restrict__ g, float* __restrict__ dx, float* __restrict__ inv) {
   __shared__ float red[4];
   const int i = blockIdx.x, tid = threadIdx.x;
@@ -560,14 +562,14 @@ __global__ void vit_grad_scale_kernel(const float* __restrict__ g, float* __rest
   if ((tid & 31) == 0) red[tid >> 5] = m;
   __syncthreads();
   m = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
-  float s = 1.f;
+  int k = 0;
   if (m > 0.f && isfinite(m)) {
     int e;
     frexpf(m, &e);               // m = f 2^e, f in [0.5, 1)
-    s = ldexpf(1.f, 1 - e);
+    k = 1 - e;
   }
-  for (int c = tid; c < kD; c += 128) dx[i * kD + c] = g[i * kD + c] * s;
-  if (tid == 0) inv[i] = 1.f / s;
+  for (int c = tid; c < kD; c += 128) dx[i * kD + c] = ldexpf(g[i * kD + c], k);
+  if (tid == 0) inv[i] = ldexpf(1.f, -k);
 }
 
 // ------------------------------------------------------------------ workspace
