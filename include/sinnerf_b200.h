@@ -115,7 +115,13 @@ int snb_field_forward(const void* packed, int precision, const float* rays, cons
 
 /* models/rendering.py:215-248.  raw (N,S,4) (raw_channels=4) or sigma (N,S) (raw_channels=1);
  * noise (N,S) standard-normal draws or NULL (treated as 0; the reference scales by noise_std).
- * rgb (N,3) / depth (N,) may be NULL with raw_channels==1 (weights_only branch :237-238). */
+ * rgb (N,3) / depth (N,) may be NULL with raw_channels==1 (weights_only branch :237-238).
+ * Alignment: with raw_channels == 4 every compositing entry point (forward, _scatter, _loss, and the backwards, for
+ * raw AND g_raw) reads / writes the [r, g, b, sigma] rows as 16-byte words: raw and g_raw must be 16-byte aligned,
+ * SNB_ERR_INVALID otherwise.  z_vals, noise, weights, g_weights and the (N,S) sigma / g_sigma rows of raw_channels == 1
+ * may have any 4-byte alignment: 16-byte aligned rows of S % 4 == 0, S <= 128 samples take the four-samples-per-thread
+ * kernels, everything else the warp-per-ray kernels, with the same results up to the association of the running
+ * product. */
 int snb_composite_forward(const float* raw, int raw_channels, const float* z_vals, const float* rays,
                           const float* noise, float noise_std, int white_back, int64_t n_rays,
                           int n_samples, float* rgb, float* depth, float* weights, void* stream);
@@ -225,7 +231,8 @@ int snb_composite_forward_loss(const float* raw, const float* z_vals, const floa
  * derivative of g_loss[0] loss[0] + g_loss[1] loss[1] (g_loss: device (2,), NULL = ones; `loss` may be NULL),
  * formed per ray in registers from the forward's rgb / depth outputs -- no (N,3)/(N,) gradient tensors and
  * no elementwise loss kernels.  g_amax (nullable): one 32-bit word, atomically raised to the bit pattern of
- * max |g_raw| (zero it first) -- the scale statistic of the 16-bit field backward. */
+ * max |g_raw| (zero it first) -- the scale statistic of the 16-bit field backward.  An infinite gradient leaves the
+ * pattern of 3.0e38f; NaN gradients are skipped (the word is the maximum over the others). */
 int snb_composite_backward_loss(const float* raw, const float* z_vals, const float* rays, const float* noise,
                                 float noise_std, int white_back, const float* g_rgb, const float* g_depth,
                                 const float* g_weights, const SnbLossSpec* loss, const float* rgb, const float* depth,

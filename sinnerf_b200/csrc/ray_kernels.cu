@@ -426,7 +426,9 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(
   if (g_amax != nullptr) {
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) amax = fmaxf(amax, __shfl_xor_sync(kFull, amax, off));
-    // non-negative floats order like their bit patterns; NaN / inf gradients saturate the statistic
+    // non-negative floats order like their bit patterns.  An infinite gradient saturates the statistic; a NaN one is
+    // skipped (fmaxf returns its other operand), so the word holds the maximum over the non-NaN gradients and amax is
+    // never NaN here -- the 16-bit backward turns a NaN gradient into NaN at any scale, so no scale is chosen for it
     if (lane == 0 && amax > 0.f) atomicMax(g_amax, __float_as_uint(amax == amax ? fminf(amax, 3.0e38f) : 3.0e38f));
   }
 }
@@ -679,7 +681,9 @@ __global__ void __launch_bounds__(256) composite_bwd4_kernel(
   if (g_amax != nullptr) {
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) amax = fmaxf(amax, __shfl_xor_sync(kFull, amax, off));
-    // non-negative floats order like their bit patterns; NaN / inf gradients saturate the statistic
+    // non-negative floats order like their bit patterns.  An infinite gradient saturates the statistic; a NaN one is
+    // skipped (fmaxf returns its other operand), so the word holds the maximum over the non-NaN gradients and amax is
+    // never NaN here -- the 16-bit backward turns a NaN gradient into NaN at any scale, so no scale is chosen for it
     if (lane == 0 && amax > 0.f) atomicMax(g_amax, __float_as_uint(amax == amax ? fminf(amax, 3.0e38f) : 3.0e38f));
   }
 }
