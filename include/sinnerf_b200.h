@@ -376,6 +376,47 @@ int snb_vit_forward(const void* image, int precision, const float* const* images
 int snb_vit_backward(const void* image, int precision, const int* sizes, int n_images, const float* d_out,
                      float* const* d_images, const int64_t* d_strides, void* workspace, void* stream);
 
+/* ---- adversarial loss: spectral-norm patch discriminator with DiffAugment ----------------------------
+ * models/discriminator.py Discriminator(conditional=False, policy='color,cutout', ndf=64, imsize): 4 x 4
+ * convolutions without bias, each weight torch.nn.utils.spectral_norm(n_power_iterations=1, eps=1e-12) of its
+ * weight_orig viewed as (out, in 16); stride 2 pad 1 and LeakyReLU(0.2), with InstanceNorm2d (eps 1e-5, no affine,
+ * instance statistics) before the LeakyReLU where the branch has one; the last convolution (512 -> 1) has stride 1,
+ * pad 0.  Branches by imsize (layers, channels):
+ *   128: 6, 3-32-64-128-256-512-1, IN after layers 2-5     64: 5, 3-64-128-256-512-1, IN after layers 2-4
+ *    32: 4, 3-128-256-512-1, IN after layers 1-3           any other imsize: 3, 3-256-512-1, IN after layers 1-2
+ * weights: HOST array of the branch's layer count of device pointers to the fp32 weight_orig tensors (contiguous,
+ * (out, in, 4, 4)); weight_u / weight_v: HOST arrays of device pointers to the spectral_norm buffers.  training = 1
+ * runs one power iteration v = normalize(W^T u), u = normalize(W v) and writes u, v in place (as torch does in
+ * training mode); training = 0 uses them unchanged.  sigma = u . W v either way, on the device.
+ * input: (n, 3, height, width) fp32 read through strides (HOST, 4: image, channel, row, column).  aug: NULL, or
+ * brightness NULL: no augmentation; else DiffAugment's color and cutout draws (device, n each):
+ *   x + (brightness - 0.5); saturation about the per-pixel channel mean, factor 2 saturation; contrast about the
+ *   per-image mean, factor contrast + 0.5; zero rows clamp(cutout_y - ch/2 .. + ch - 1) x columns
+ *   clamp(cutout_x - cw/2 .. + cw - 1), ch = (int)(height / 2 + 0.5), cw likewise.
+ * out: (n, 1, oh, ow), contiguous.  The arithmetic of every convolution GEMM is `precision` (SNB_PREC_*, as for
+ * the ViT).  workspace: snb_disc_workspace_bytes(imsize, n, height, width, save) bytes, any content; save = 1 adds
+ * the backward's scratch.  The call makes no host synchronisation. */
+#define SNB_DISC_MAX_LAYERS 6
+typedef struct SnbDiscAug {
+  const float* brightness;   /* (n,) torch.rand draws; NULL = no augmentation */
+  const float* saturation;   /* (n,) */
+  const float* contrast;     /* (n,) */
+  const int64_t* cutout_y;   /* (n,) torch.randint offset along the rows */
+  const int64_t* cutout_x;   /* (n,) ... along the columns */
+} SnbDiscAug;
+/* 0 for a shape the branch cannot run (a convolution with an empty output, an InstanceNorm over one element) */
+size_t snb_disc_workspace_bytes(int imsize, int n, int height, int width, int save);
+int snb_disc_forward(int imsize, int precision, int training, const float* const* weights, float* const* weight_u,
+                     float* const* weight_v, const float* input, const int64_t* strides, int n, int height, int width,
+                     const SnbDiscAug* aug, float* out, void* workspace, void* stream);
+/* Gradients of the forward whose workspace (save = 1 size) this is, with respect to its input (d_input NULL: not
+ * wanted; written through d_strides, every element) and to each weight_orig (d_weights: HOST array, NULL entries
+ * not wanted; each written, not accumulated), from d_out (n, 1, oh, ow) contiguous.  The forward's own sigma, u and
+ * v are used.  The workspace's saved part is only read, so the call may be repeated. */
+int snb_disc_backward(int imsize, int precision, const float* const* weights, int n, int height, int width,
+                      const float* d_out, float* d_input, const int64_t* d_strides, float* const* d_weights,
+                      void* workspace, void* stream);
+
 /* ---- optimiser step (SURVEY.md 8f-4) --------------------------------------------------------------
  * torch.optim.Adam as the reference configures it (utils/__init__.py:19-21: lr, eps = 1e-8, weight_decay;
  * betas default (0.9, 0.999), amsgrad off), fused over the 24 parameter tensors of one NeRF, followed on the

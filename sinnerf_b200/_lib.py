@@ -62,6 +62,12 @@ class SnbOptimArgs(C.Structure):
                 ("alpha", C.c_double), ("k", C.c_int), ("step", C.c_int * 24)]
 
 
+class SnbDiscAug(C.Structure):
+    _fields_ = [("brightness", c_f), ("saturation", c_f), ("contrast", c_f), ("cutout_y", c_f), ("cutout_x", c_f)]
+
+
+DISC_MAX_LAYERS = 6   # SNB_DISC_MAX_LAYERS
+
 LOSS_WS_FLOATS = 4096   # SNB_LOSS_WS_FLOATS
 PARAM_FLOATS = 595844   # SNB_PARAM_FLOATS
 
@@ -130,6 +136,12 @@ SIGNATURES = {
                                   C.c_int, C.c_int, c_f, c_f, c_f]),
     "snb_vit_backward": (C.c_int, [c_f, C.c_int, C.POINTER(C.c_int), C.c_int, c_f, C.POINTER(C.c_void_p),
                                    C.POINTER(C.c_int64), c_f, c_f]),
+    "snb_disc_workspace_bytes": (C.c_size_t, [C.c_int] * 5),
+    "snb_disc_forward": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                   C.POINTER(C.c_void_p), c_f, C.POINTER(C.c_int64), C.c_int, C.c_int, C.c_int,
+                                   C.POINTER(SnbDiscAug), c_f, c_f, c_f]),
+    "snb_disc_backward": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, c_f, c_f,
+                                    C.POINTER(C.c_int64), C.POINTER(C.c_void_p), c_f, c_f]),
 }
 VIT_N_TENSORS = 148       # SNB_VIT_N_TENSORS
 VIT_MAX_IMAGES = 8        # SNB_VIT_MAX_IMAGES

@@ -18,7 +18,7 @@ LIB = os.path.join(PKG, "libsinnerf_b200.so")
 STAMP = os.path.join(PKG, ".libsinnerf_b200.stamp")
 
 SOURCES = ["api.cu", "ray_kernels.cu", "field_simt.cu", "field_tc.cu", "field_bwd.cu", "wgrad_tc.cu", "dgrad_tc.cu", "optim.cu",
-           "wgrad16.cu", "dgrad16.cu", "bwd16.cu", "patch_loss.cu", "warp.cu", "vit.cu"]
+           "wgrad16.cu", "dgrad16.cu", "bwd16.cu", "patch_loss.cu", "warp.cu", "vit.cu", "disc.cu"]
 HEADERS = ["common.cuh", os.path.join(ROOT, "include", "sinnerf_b200.h")]
 
 NVCC_FLAGS = [
