@@ -462,6 +462,28 @@ int snb_optim_step(float* const* params, const float* const* grads, float* exp_a
                    float* slow_buffer, const SnbOptimArgs* args, int precision, int new_activation, void* packed,
                    void* stream);
 
+/* One step of args->rule over a table of n plain fp32 tensors (the discriminator's weight_orig tensors, stepped by
+ * get_optimizer(hparams, [D], rate=0.2)), in one launch, with no checksum stamp and no re-pack.  Same element
+ * arithmetic as snb_adam_step (SNB_OPTIM_ADAM, which only this entry point takes: torch.optim.Adam's single-tensor
+ * path with its per-parameter step) and snb_optim_step (SGD / RAdam / Ranger).
+ *   params, grads, numel, step: HOST arrays of n entries (1 <= n <= SNB_OPTIM_MAX_TENSORS).  params[i]: device
+ *     pointer to numel[i] >= 1 contiguous floats, updated in place.  grads[i]: device pointer, or NULL = no gradient
+ *     (the tensor neither moves nor touches its state).  step[i]: tensor i's update count including this one (for
+ *     SGD: the momentum-buffer update count, 0 allowed when momentum == 0); ignored where grads[i] is NULL.
+ *   exp_avg / exp_avg_sq / slow_buffer: device buffers of sum(numel) floats, tensor i's state at offset
+ *     sum(numel[0..i)).  Needed: Adam / RAdam exp_avg and exp_avg_sq; Ranger all three; SGD exp_avg when
+ *     momentum != 0 (the momentum buffer).  The others may be NULL.
+ *   args: rule (SNB_OPTIM_*) and hyper-parameters as for snb_optim_step; args->step is not read.
+ * Scalars depending on a tensor's step (bias corrections, N_sma / step_size, the Ranger sync) are formed per tensor
+ * on the host in double, in the reference's expression order.  Each element is updated independently, so repeated
+ * calls on the same inputs give the same bits.  SNB_ERR_INVALID for null tables, n out of range, numel <= 0, a null
+ * parameter, a null buffer the rule needs, a step count below 1 where it is read, and invalid hyper-parameters. */
+#define SNB_OPTIM_ADAM 3
+#define SNB_OPTIM_MAX_TENSORS 32
+int snb_optim_step_tensors(int n, float* const* params, const float* const* grads, const int64_t* numel,
+                           const int* step, float* exp_avg, float* exp_avg_sq, float* slow_buffer,
+                           const SnbOptimArgs* args, void* stream);
+
 /* ---- whole path -------------------------------------------------------------------- */
 typedef struct SnbRenderArgs {
   const float* rays;        /* (N,8)                                                    */

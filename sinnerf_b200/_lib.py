@@ -53,7 +53,8 @@ class SnbAdamArgs(C.Structure):
                 ("weight_decay", C.c_double), ("step", C.c_int)]
 
 
-OPTIM_SGD, OPTIM_RADAM, OPTIM_RANGER = 0, 1, 2   # SNB_OPTIM_*
+OPTIM_SGD, OPTIM_RADAM, OPTIM_RANGER, OPTIM_ADAM = 0, 1, 2, 3   # SNB_OPTIM_* (ADAM: snb_optim_step_tensors only)
+OPTIM_MAX_TENSORS = 32   # SNB_OPTIM_MAX_TENSORS
 
 
 class SnbOptimArgs(C.Structure):
@@ -109,6 +110,8 @@ SIGNATURES = {
                                 C.c_int, C.c_int, c_f, c_f]),
     "snb_optim_step": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, c_f, C.POINTER(SnbOptimArgs),
                                  C.c_int, C.c_int, c_f, c_f]),
+    "snb_optim_step_tensors": (C.c_int, [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
+                                         C.POINTER(C.c_int), c_f, c_f, c_f, C.POINTER(SnbOptimArgs), c_f]),
     "snb_field_backward": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, c_f, c_f, c_f, c_f, c_f,
                                      c_f, C.c_int64, c_f, c_f, c_f, c_f, c_f, c_f]),
     "snb_field_forward_train_sigma": (C.c_int, [c_f, C.c_int, c_f, c_f, C.c_int64, C.c_int, c_f, c_f, c_f, c_f]),

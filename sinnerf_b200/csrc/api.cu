@@ -72,6 +72,8 @@ int field_backward16_sigma(const float* const*, float* const*, const float*, con
 int adam_step_pack(float* const*, const float* const*, float*, float*, const SnbAdamArgs&, int, int, void*, cudaStream_t);
 int optim_step_pack(float* const*, const float* const*, float*, float*, float*, const SnbOptimArgs&, int, int, void*,
                     cudaStream_t);
+int optim_step_tensors(int, float* const*, const float* const*, const int64_t*, const int*, float*, float*, float*,
+                       const SnbOptimArgs&, cudaStream_t);
 // tensor-core modes (field_tc.cu)
 size_t tc_packed_bytes(int precision);
 int field_forward_tc(const void*, int, const float*, const float*, int64_t, int, int, float*, cudaStream_t);
@@ -497,6 +499,34 @@ int snb_optim_step(float* const* params, const float* const* grads, float* exp_a
     if (int rc = check_precision(precision)) return rc;
   return optim_step_pack(params, grads, exp_avg, exp_avg_sq, slow_buffer, *args, precision, new_activation, packed,
                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_optim_step_tensors(int n, float* const* params, const float* const* grads, const int64_t* numel,
+                           const int* step, float* exp_avg, float* exp_avg_sq, float* slow_buffer,
+                           const SnbOptimArgs* args, void* stream) {
+  const char* who = "snb_optim_step_tensors";
+  SNB_REQUIRE(params && grads && numel && step && args, "%s: null table or args", who);
+  SNB_REQUIRE(n >= 1 && n <= SNB_OPTIM_MAX_TENSORS, "%s: needs 1 <= n <= %d tensors (got %d)", who,
+              SNB_OPTIM_MAX_TENSORS, n);
+  const int rule = args->rule;
+  SNB_REQUIRE(rule == SNB_OPTIM_SGD || rule == SNB_OPTIM_RADAM || rule == SNB_OPTIM_RANGER || rule == SNB_OPTIM_ADAM,
+              "%s: unknown rule %d", who, rule);
+  const bool sgd = rule == SNB_OPTIM_SGD;
+  SNB_REQUIRE((exp_avg != nullptr || (sgd && args->momentum == 0.)) && (sgd || exp_avg_sq != nullptr) &&
+                  (rule != SNB_OPTIM_RANGER || slow_buffer != nullptr),
+              "%s: null state buffer (rule %d)", who, rule);
+  for (int i = 0; i < n; ++i) {
+    SNB_REQUIRE(params[i] != nullptr, "%s: parameter tensor %d is null", who, i);
+    SNB_REQUIRE(numel[i] >= 1, "%s: numel of tensor %d must be >= 1 (got %lld)", who, i, (long long)numel[i]);
+    SNB_REQUIRE(grads[i] == nullptr || step[i] >= 1 || (sgd && args->momentum == 0.),
+                "%s: step of tensor %d counts from 1 (got %d)", who, i, step[i]);
+  }
+  SNB_REQUIRE(args->lr >= 0. && args->weight_decay >= 0. && args->momentum >= 0. && args->eps >= 0. &&
+                  args->beta1 >= 0. && args->beta1 < 1. && args->beta2 >= 0. && args->beta2 < 1. &&
+                  args->alpha >= 0. && args->alpha <= 1. && args->k >= 1,
+              "%s: invalid hyper-parameters", who);
+  return optim_step_tensors(n, params, grads, numel, step, exp_avg, exp_avg_sq, slow_buffer, *args,
+                            reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_depth_smooth_forward(const float* idepth, const int64_t* idepth_strides, const float* image,

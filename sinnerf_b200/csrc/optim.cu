@@ -50,6 +50,19 @@ __device__ __forceinline__ void stamp_checksum(unsigned long long h, PackedHeade
   }
 }
 
+// One element of torch.optim.Adam's single-tensor step (the arithmetic listed above): m and v in, updated m, v and
+// the new parameter out.  Shared by the NeRF kernel and the table walker (optim_tensors_kernel).
+__device__ __forceinline__ float adam_update(float w, float gr, float& m, float& v, float lr_neg_step, float beta1_w,
+                                             float beta2, float beta2_w, float eps, float weight_decay,
+                                             float inv_bc2_sqrt) {
+  if (weight_decay != 0.f) gr = fmaf(weight_decay, w, gr);
+  m = fmaf(beta1_w, gr - m, m);
+  v = __fmul_rn(v, beta2);
+  v = fmaf(__fmul_rn(beta2_w, gr), gr, v);
+  const float den = __fadd_rn(__fmul_rn(__fsqrt_rn(v), inv_bc2_sqrt), eps);
+  return fmaf(lr_neg_step, __fdiv_rn(m, den), w);
+}
+
 __global__ void __launch_bounds__(256) adam_step_kernel(AdamPtrs a, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
                                                         float lr_neg_step, float beta1_w, float beta2, float beta2_w, float eps,
                                                         float weight_decay, float inv_bc2_sqrt, int precision, int new_activation,
@@ -63,14 +76,8 @@ __global__ void __launch_bounds__(256) adam_step_kernel(AdamPtrs a, float* __res
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
       float w = p[e];
       if (g != nullptr) {
-        float gr = g[e];
-        if (weight_decay != 0.f) gr = fmaf(weight_decay, w, gr);
         float m = exp_avg[base + e], v = exp_avg_sq[base + e];
-        m = fmaf(beta1_w, gr - m, m);
-        v = __fmul_rn(v, beta2);
-        v = fmaf(__fmul_rn(beta2_w, gr), gr, v);
-        const float den = __fadd_rn(__fmul_rn(__fsqrt_rn(v), inv_bc2_sqrt), eps);
-        w = fmaf(lr_neg_step, __fdiv_rn(m, den), w);
+        w = adam_update(w, g[e], m, v, lr_neg_step, beta1_w, beta2, beta2_w, eps, weight_decay, inv_bc2_sqrt);
         exp_avg[base + e] = m;
         exp_avg_sq[base + e] = v;
         p[e] = w;
@@ -91,15 +98,21 @@ static int repack(float* const* params, int precision, int new_activation, void*
   return launch_pack_tc(cp, precision, new_activation ? 1 : 0, packed, 0, st);
 }
 
+// Adam's step-dependent scalars exactly as torch forms them: python doubles, cast to float where the kernels consume
+// them.  -lr / (1 - beta1^t) and 1 / sqrt(1 - beta2^t).
+static void adam_bias_scalars(double lr, double beta1, double beta2, int step, float* lr_neg_step, float* inv_bc2_sqrt) {
+  const double bc1 = 1.0 - pow(beta1, (double)step);
+  const double bc2 = 1.0 - pow(beta2, (double)step);
+  *lr_neg_step = (float)(-(lr / bc1));
+  *inv_bc2_sqrt = 1.0f / (float)sqrt(bc2);
+}
+
 int adam_step_pack(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
                    const SnbAdamArgs& o, int precision, int new_activation, void* packed, cudaStream_t st) {
   AdamPtrs a;
   for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) { a.p[i] = params[i]; a.g[i] = grads[i]; }
-  // scalars exactly as torch forms them: python doubles, cast to float where the kernels consume them
-  const double bc1 = 1.0 - pow(o.beta1, (double)o.step);
-  const double bc2 = 1.0 - pow(o.beta2, (double)o.step);
-  const float lr_neg_step = (float)(-(o.lr / bc1));
-  const float inv_bc2_sqrt = 1.0f / (float)sqrt(bc2);
+  float lr_neg_step, inv_bc2_sqrt;
+  adam_bias_scalars(o.lr, o.beta1, o.beta2, o.step, &lr_neg_step, &inv_bc2_sqrt);
   const float beta1_w = (float)(1.0 - o.beta1), beta2_w = (float)(1.0 - o.beta2);
   adam_step_kernel<<<sm_count() * 2, 256, 0, st>>>(a, exp_avg, exp_avg_sq, lr_neg_step, beta1_w, (float)o.beta2, beta2_w,
                                                   (float)o.eps, (float)o.weight_decay, inv_bc2_sqrt, precision, new_activation,
@@ -125,14 +138,55 @@ int adam_step_pack(float* const* params, const float* const* grads, float* exp_a
 //   with slow = p (before the update) on the tensor's first step.
 enum : unsigned { kFirst = 1u, kAdaptive = 2u, kSync = 4u };
 
-struct RuleScalars {
+struct RuleConsts {
   float lr_neg;         // SGD: -lr
-  float decay;          // SGD: weight_decay;  RAdam / Ranger: -weight_decay * lr
+  float decay;          // SGD / Adam: weight_decay;  RAdam / Ranger: -weight_decay * lr
   float momentum;       // SGD
   float beta1, beta1_w, beta2, beta2_w, eps, alpha;
+};
+
+struct RuleScalars {
+  RuleConsts c;
   float step_lr[SNB_N_PARAM_TENSORS];           // RAdam / Ranger: -step_size * lr at the tensor's own step
   unsigned char flags[SNB_N_PARAM_TENSORS];     // kFirst | kAdaptive | kSync
 };
+
+// One element of SGD / RAdam / Ranger (the arithmetic listed above) at flat state index i: reads and writes the state
+// buffers the rule keeps and returns the new parameter.  Shared by optim_step_kernel and optim_tensors_kernel.
+template <int RULE>
+__device__ __forceinline__ float rule_update(float w, float gr, unsigned long long i, float* __restrict__ exp_avg,
+                                             float* __restrict__ exp_avg_sq, float* __restrict__ slow_buffer,
+                                             const RuleConsts& s, unsigned f, float step_lr) {
+  if (RULE == SNB_OPTIM_SGD) {
+    if (s.decay != 0.f) gr = fmaf(s.decay, w, gr);
+    if (s.momentum != 0.f) {
+      if (!(f & kFirst)) gr = __fadd_rn(__fmul_rn(exp_avg[i], s.momentum), gr);
+      exp_avg[i] = gr;
+    }
+    return fmaf(s.lr_neg, gr, w);
+  }
+  float v = __fmul_rn(exp_avg_sq[i], s.beta2);
+  v = fmaf(__fmul_rn(s.beta2_w, gr), gr, v);
+  float m = __fmul_rn(exp_avg[i], s.beta1);
+  m = fmaf(s.beta1_w, gr, m);
+  exp_avg[i] = m;
+  exp_avg_sq[i] = v;
+  float slow = 0.f;
+  if (RULE == SNB_OPTIM_RANGER) slow = (f & kFirst) ? w : slow_buffer[i];
+  if (s.decay != 0.f) w = fmaf(s.decay, w, w);
+  if (f & kAdaptive)
+    w = fmaf(step_lr, __fdiv_rn(m, __fadd_rn(__fsqrt_rn(v), s.eps)), w);
+  else
+    w = fmaf(step_lr, m, w);
+  if (RULE == SNB_OPTIM_RANGER) {
+    if (f & kSync) {
+      slow = fmaf(s.alpha, __fsub_rn(w, slow), slow);
+      w = slow;
+    }
+    if (f & (kFirst | kSync)) slow_buffer[i] = slow;
+  }
+  return w;
+}
 
 template <int RULE>
 __global__ void __launch_bounds__(256) optim_step_kernel(AdamPtrs a, float* __restrict__ exp_avg,
@@ -149,37 +203,7 @@ __global__ void __launch_bounds__(256) optim_step_kernel(AdamPtrs a, float* __re
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
       float w = p[e];
       if (g != nullptr) {
-        float gr = g[e];
-        const unsigned long long i = base + e;
-        if (RULE == SNB_OPTIM_SGD) {
-          if (s.decay != 0.f) gr = fmaf(s.decay, w, gr);
-          if (s.momentum != 0.f) {
-            if (!(f & kFirst)) gr = __fadd_rn(__fmul_rn(exp_avg[i], s.momentum), gr);
-            exp_avg[i] = gr;
-          }
-          w = fmaf(s.lr_neg, gr, w);
-        } else {
-          float v = __fmul_rn(exp_avg_sq[i], s.beta2);
-          v = fmaf(__fmul_rn(s.beta2_w, gr), gr, v);
-          float m = __fmul_rn(exp_avg[i], s.beta1);
-          m = fmaf(s.beta1_w, gr, m);
-          exp_avg[i] = m;
-          exp_avg_sq[i] = v;
-          float slow = 0.f;
-          if (RULE == SNB_OPTIM_RANGER) slow = (f & kFirst) ? w : slow_buffer[i];
-          if (s.decay != 0.f) w = fmaf(s.decay, w, w);
-          if (f & kAdaptive)
-            w = fmaf(step_lr, __fdiv_rn(m, __fadd_rn(__fsqrt_rn(v), s.eps)), w);
-          else
-            w = fmaf(step_lr, m, w);
-          if (RULE == SNB_OPTIM_RANGER) {
-            if (f & kSync) {
-              slow = fmaf(s.alpha, __fsub_rn(w, slow), slow);
-              w = slow;
-            }
-            if (f & (kFirst | kSync)) slow_buffer[i] = slow;
-          }
-        }
+        w = rule_update<RULE>(w, g[e], base + e, exp_avg, exp_avg_sq, slow_buffer, s.c, f, step_lr);
         p[e] = w;
       }
       h += param_checksum_term(base + e, __float_as_uint(w));
@@ -189,41 +213,57 @@ __global__ void __launch_bounds__(256) optim_step_kernel(AdamPtrs a, float* __re
   stamp_checksum(h, hdr);
 }
 
+static RuleConsts rule_consts(const SnbOptimArgs& o) {
+  RuleConsts c = {};
+  if (o.rule == SNB_OPTIM_SGD) {
+    c.lr_neg = (float)(-o.lr);
+    c.decay = (float)o.weight_decay;
+    c.momentum = (float)o.momentum;
+    return c;
+  }
+  c.beta1 = (float)o.beta1;
+  c.beta1_w = (float)(1.0 - o.beta1);
+  c.beta2 = (float)o.beta2;
+  c.beta2_w = (float)(1.0 - o.beta2);
+  c.eps = (float)o.eps;
+  c.alpha = (float)o.alpha;
+  c.decay = o.rule == SNB_OPTIM_ADAM ? (float)o.weight_decay : (float)(-o.weight_decay * o.lr);
+  return c;
+}
+
+// SGD / RAdam / Ranger: the flags and -step_size * lr of a tensor at its own step count (its update count including
+// this one).  RAdam / Ranger: utils/optimizers.py:68-86 / :397-411 in python doubles, the reference's expression order.
+static void rule_tensor_scalars(const SnbOptimArgs& o, int step, float* step_lr, unsigned* flags) {
+  if (o.rule == SNB_OPTIM_SGD) {
+    *step_lr = 0.f;
+    *flags = step == 1 ? kFirst : 0u;
+    return;
+  }
+  const double beta2_t = pow(o.beta2, (double)step);
+  const double n_sma_max = 2 / (1 - o.beta2) - 1;
+  const double n_sma = n_sma_max - 2 * step * beta2_t / (1 - beta2_t);
+  const bool adaptive = o.rule == SNB_OPTIM_RADAM ? n_sma >= 5 : n_sma > o.n_sma_threshold;
+  const double step_size =
+      adaptive ? sqrt((1 - beta2_t) * (n_sma - 4) / (n_sma_max - 4) * (n_sma - 2) / n_sma * n_sma_max /
+                      (n_sma_max - 2)) / (1 - pow(o.beta1, (double)step))
+               : 1.0 / (1 - pow(o.beta1, (double)step));
+  *step_lr = (float)(-step_size * o.lr);
+  *flags = (adaptive ? kAdaptive : 0u) | (step == 1 ? kFirst : 0u) |
+           (o.rule == SNB_OPTIM_RANGER && step % o.k == 0 ? kSync : 0u);
+}
+
 int optim_step_pack(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
                     float* slow_buffer, const SnbOptimArgs& o, int precision, int new_activation, void* packed,
                     cudaStream_t st) {
   AdamPtrs a;
   for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) { a.p[i] = params[i]; a.g[i] = grads[i]; }
   RuleScalars s = {};
-  if (o.rule == SNB_OPTIM_SGD) {
-    s.lr_neg = (float)(-o.lr);
-    s.decay = (float)o.weight_decay;
-    s.momentum = (float)o.momentum;
-    for (int t = 0; t < SNB_N_PARAM_TENSORS; ++t) s.flags[t] = o.step[t] == 1 ? kFirst : 0u;
-  } else {
-    s.beta1 = (float)o.beta1;
-    s.beta1_w = (float)(1.0 - o.beta1);
-    s.beta2 = (float)o.beta2;
-    s.beta2_w = (float)(1.0 - o.beta2);
-    s.eps = (float)o.eps;
-    s.alpha = (float)o.alpha;
-    s.decay = (float)(-o.weight_decay * o.lr);
-    for (int t = 0; t < SNB_N_PARAM_TENSORS; ++t) {
-      if (grads[t] == nullptr) continue;
-      // utils/optimizers.py:68-86 / :397-411 in python doubles, the reference's expression order
-      const int step = o.step[t];
-      const double beta2_t = pow(o.beta2, (double)step);
-      const double n_sma_max = 2 / (1 - o.beta2) - 1;
-      const double n_sma = n_sma_max - 2 * step * beta2_t / (1 - beta2_t);
-      const bool adaptive = o.rule == SNB_OPTIM_RADAM ? n_sma >= 5 : n_sma > o.n_sma_threshold;
-      const double step_size =
-          adaptive ? sqrt((1 - beta2_t) * (n_sma - 4) / (n_sma_max - 4) * (n_sma - 2) / n_sma * n_sma_max /
-                          (n_sma_max - 2)) / (1 - pow(o.beta1, (double)step))
-                   : 1.0 / (1 - pow(o.beta1, (double)step));
-      s.step_lr[t] = (float)(-step_size * o.lr);
-      s.flags[t] = (adaptive ? kAdaptive : 0u) | (step == 1 ? kFirst : 0u) |
-                   (o.rule == SNB_OPTIM_RANGER && step % o.k == 0 ? kSync : 0u);
-    }
+  s.c = rule_consts(o);
+  for (int t = 0; t < SNB_N_PARAM_TENSORS; ++t) {
+    if (o.rule != SNB_OPTIM_SGD && grads[t] == nullptr) continue;
+    unsigned f;
+    rule_tensor_scalars(o, o.step[t], &s.step_lr[t], &f);
+    s.flags[t] = (unsigned char)f;
   }
   PackedHeader* hdr = reinterpret_cast<PackedHeader*>(packed);
   const int grid = sm_count() * 2;
@@ -235,6 +275,82 @@ int optim_step_pack(float* const* params, const float* const* grads, float* exp_
     optim_step_kernel<SNB_OPTIM_RANGER><<<grid, 256, 0, st>>>(a, exp_avg, exp_avg_sq, slow_buffer, s, hdr);
   if (int rc = check_launch("optim_step_kernel")) return rc;
   return repack(params, precision, new_activation, packed, st);
+}
+
+// ---------------------------------------------------------------- any tensors (snb_optim_step_tensors)
+// The four rules over a caller-given table of plain fp32 tensors (the discriminator's weight_orig): no checksum and no
+// re-pack.  Tensor t's state sits at offset sum(numel[0..t)) of each flat buffer.  Tensors without a gradient are
+// left out of the table on the host, so every entry is updated.
+struct TensorEntry {
+  float* p;
+  const float* g;
+  long long n;
+  unsigned long long off;   // the tensor's offset in the flat state buffers
+  float step_lr;            // Adam: -lr / (1 - beta1^t);  RAdam / Ranger: -step_size * lr
+  float inv_bc2_sqrt;       // Adam: 1 / sqrt(1 - beta2^t)
+  unsigned flags;           // SGD / RAdam / Ranger: kFirst | kAdaptive | kSync
+};
+
+struct TensorTable {
+  TensorEntry t[SNB_OPTIM_MAX_TENSORS];
+  int n;
+};
+
+template <int RULE>
+__global__ void __launch_bounds__(256) optim_tensors_kernel(TensorTable tab, float* __restrict__ exp_avg,
+                                                            float* __restrict__ exp_avg_sq,
+                                                            float* __restrict__ slow_buffer, RuleConsts c) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (int t = 0; t < tab.n; ++t) {
+    float* p = tab.t[t].p;
+    const float* g = tab.t[t].g;
+    const long long n = tab.t[t].n;
+    const unsigned long long off = tab.t[t].off;
+    const float step_lr = tab.t[t].step_lr;
+    const float inv_bc2_sqrt = tab.t[t].inv_bc2_sqrt;
+    const unsigned f = tab.t[t].flags;
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += stride) {
+      const unsigned long long i = off + e;
+      if (RULE == SNB_OPTIM_ADAM) {
+        float m = exp_avg[i], v = exp_avg_sq[i];
+        p[e] = adam_update(p[e], g[e], m, v, step_lr, c.beta1_w, c.beta2, c.beta2_w, c.eps, c.decay, inv_bc2_sqrt);
+        exp_avg[i] = m;
+        exp_avg_sq[i] = v;
+      } else {
+        p[e] = rule_update<RULE>(p[e], g[e], i, exp_avg, exp_avg_sq, slow_buffer, c, f, step_lr);
+      }
+    }
+  }
+}
+
+int optim_step_tensors(int n, float* const* params, const float* const* grads, const int64_t* numel, const int* step,
+                       float* exp_avg, float* exp_avg_sq, float* slow_buffer, const SnbOptimArgs& o, cudaStream_t st) {
+  TensorTable tab = {};
+  unsigned long long off = 0;
+  for (int t = 0; t < n; off += (unsigned long long)numel[t], ++t) {
+    if (grads[t] == nullptr) continue;
+    TensorEntry& te = tab.t[tab.n++];
+    te.p = params[t];
+    te.g = grads[t];
+    te.n = numel[t];
+    te.off = off;
+    if (o.rule == SNB_OPTIM_ADAM)
+      adam_bias_scalars(o.lr, o.beta1, o.beta2, step[t], &te.step_lr, &te.inv_bc2_sqrt);
+    else
+      rule_tensor_scalars(o, step[t], &te.step_lr, &te.flags);
+  }
+  if (tab.n == 0) return SNB_OK;
+  const RuleConsts c = rule_consts(o);
+  const int grid = sm_count() * 4;
+  if (o.rule == SNB_OPTIM_ADAM)
+    optim_tensors_kernel<SNB_OPTIM_ADAM><<<grid, 256, 0, st>>>(tab, exp_avg, exp_avg_sq, slow_buffer, c);
+  else if (o.rule == SNB_OPTIM_SGD)
+    optim_tensors_kernel<SNB_OPTIM_SGD><<<grid, 256, 0, st>>>(tab, exp_avg, exp_avg_sq, slow_buffer, c);
+  else if (o.rule == SNB_OPTIM_RADAM)
+    optim_tensors_kernel<SNB_OPTIM_RADAM><<<grid, 256, 0, st>>>(tab, exp_avg, exp_avg_sq, slow_buffer, c);
+  else
+    optim_tensors_kernel<SNB_OPTIM_RANGER><<<grid, 256, 0, st>>>(tab, exp_avg, exp_avg_sq, slow_buffer, c);
+  return check_launch("optim_tensors_kernel");
 }
 
 }  // namespace snb

@@ -11,98 +11,61 @@ fp32 buffer per model; `state_dict()` exposes per-parameter views with torch.opt
 `FusedSGD`, `FusedRAdam` and `FusedRanger` do the same for the reference's other `--optimizer` choices (torch.optim.SGD,
 and the reference's own RAdam and Ranger, utils/optimizers.py), with per-parameter step counts and state keys as
 those optimizers keep them, so checkpoints move both ways between them and the fused ones.
+
+All four also step `sinnerf_b200.discriminator.Discriminator` modules, which `get_optimizer(hparams, [self.D],
+rate=0.2)` hands them for the adversarial loss (models/sinnerf.py:207-209): every weight_orig of a module in one
+launch of snb_optim_step_tensors, with no re-pack (the discriminator derives its GEMM copy of each weight on every
+call).  There Adam too keeps a step count per parameter, and every rule creates a parameter's state on its first step,
+as torch.optim.Adam / SGD and the reference's RAdam / Ranger do over `D.parameters()`; so `opt_d`'s state dict moves
+both ways between them and the fused optimisers.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Iterable, List, Optional
+from typing import Iterable, Optional
 
 import torch
 
 from . import _lib, config
+from .discriminator import Discriminator
 from .nerf import NeRF
 
 __all__ = ["FusedAdam", "FusedSGD", "FusedRAdam", "FusedRanger", "get_optimizer"]
 
 
-class FusedAdam(torch.optim.Optimizer):
-    def __init__(self, models: Iterable[NeRF], lr: float = 5e-4, betas=(0.9, 0.999), eps: float = 1e-8,
-                 weight_decay: float = 0.0, precision: Optional[str] = None):
-        self.models: List[NeRF] = list(models)
-        if not self.models or not all(isinstance(m, NeRF) for m in self.models):
-            raise TypeError("FusedAdam steps sinnerf_b200.NeRF models (pass the modules, not their parameters)")
-        params = [p for m in self.models for p in m._param_list()]
-        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
-        self._precision = precision
-        self._flat = []          # per model: (exp_avg, exp_avg_sq) flat device buffers
-        self._steps = 0
+def _check_modules(models, who: str):
+    """(the modules as a list, whether they are Discriminators); TypeError unless they are all NeRF models or all
+    Discriminators."""
+    models = list(models)
+    for kind in (NeRF, Discriminator):
+        if models and all(isinstance(m, kind) for m in models):
+            return models, kind is Discriminator
+    raise TypeError(f"{who} steps sinnerf_b200.NeRF models or sinnerf_b200.discriminator.Discriminator modules, all "
+                    "of one kind (pass the modules, not their parameters)")
 
-    def _ensure_state(self):
-        if self._flat:
-            return
-        for m in self.models:
-            ps = m._param_list()
-            dev = ps[0].device
-            _lib.require_device(ps[0], "FusedAdam")
-            ea = torch.zeros(_lib.PARAM_FLOATS, device=dev, dtype=torch.float32)
-            es = torch.zeros(_lib.PARAM_FLOATS, device=dev, dtype=torch.float32)
-            off = 0
-            for p in ps:
-                n = p.numel()
-                self.state[p] = {"step": torch.tensor(float(self._steps)), "exp_avg": ea[off:off + n].view_as(p),
-                                 "exp_avg_sq": es[off:off + n].view_as(p)}
-                off += n
-            assert off == _lib.PARAM_FLOATS
-            self._flat.append((ea, es))
 
-    def load_state_dict(self, state_dict):
-        """Values are copied INTO the flat buffers (the kernel addresses them by offset)."""
-        self._ensure_state()
-        views = {id(p): dict(st) for p, st in self.state.items()}
-        super().load_state_dict(state_dict)
-        step = 0
-        for p, st in self.state.items():
-            keep = views[id(p)]
-            for k in ("exp_avg", "exp_avg_sq"):
-                keep[k].copy_(st[k])
-                st[k] = keep[k]
-            step = max(step, int(float(st.get("step", 0))))
-        self._steps = step
+def _params(m) -> list:
+    """The tensors a step of module m updates: a NeRF's 24 in state-dict order, a Discriminator's weight_orig tensors
+    in `parameters()` order (what the reference's get_optimizer hands torch; its convolutions have no bias and its
+    InstanceNorms no affine parameters).  Like NeRF._param_list, reads the current Parameter objects from the module
+    dicts: `parameters()` walks every submodule and costs ~20 us of host time per step."""
+    if isinstance(m, NeRF):
+        return m._param_list()
+    return [c._parameters["weight_orig"] for c in m.main._modules.values() if "weight_orig" in c._parameters]
 
-    @torch.no_grad()
-    def step(self, closure=None):
-        loss = None
-        if closure is not None:
-            with torch.enable_grad():
-                loss = closure()
-        self._ensure_state()
-        lib = _lib.load()
-        g = self.param_groups[0]
-        self._steps += 1
-        args = _lib.SnbAdamArgs(float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]),
-                                float(g["weight_decay"]), self._steps)
-        for m, (ea, es) in zip(self.models, self._flat):
-            prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
-            ps = m._param_list()
-            dev = ps[0].device
-            for p in ps:
-                if p.dtype != torch.float32 or not p.is_contiguous() or (p.grad is not None and not p.grad.is_contiguous()):
-                    raise ValueError("FusedAdam: parameters and gradients must be contiguous fp32 CUDA tensors")
-            image = m.packed_image_buffer(prec)
-            parr = (C.c_void_p * 24)(*[p.data_ptr() for p in ps])
-            garr = (C.c_void_p * 24)(*[(p.grad.data_ptr() if p.grad is not None else None) for p in ps])
-            with torch.cuda.device(dev):
-                _lib.check(lib.snb_adam_step(parr, garr, _lib.ptr(ea), _lib.ptr(es), C.byref(args), prec,
-                                             int(m.use_new_activation), _lib.ptr(image), _lib.stream_ptr(dev)),
-                           "snb_adam_step")
-        for st in self.state.values():
-            st["step"] = torch.tensor(float(self._steps))
-        return loss
+
+def _check_tensors(ps, who: str) -> None:
+    for p in ps:
+        if p.dtype != torch.float32 or not p.is_contiguous() or (p.grad is not None and not p.grad.is_contiguous()):
+            raise ValueError(f"{who}: parameters and gradients must be contiguous fp32 CUDA tensors")
+        if p.device != ps[0].device:
+            raise ValueError(f"{who}: a module's parameters must be on one device (got {p.device} and {ps[0].device})")
 
 
 class _FusedPerTensor(torch.optim.Optimizer):
     """Shared body of FusedSGD / FusedRAdam / FusedRanger (C ABI snb_optim_step): one kernel per model and step, then
-    the re-pack of the weight image on the same stream.
+    the re-pack of the weight image on the same stream.  For Discriminator modules (and FusedAdam over them): one
+    snb_optim_step_tensors launch per module and step, nothing to re-pack.
 
     These rules keep a step count per parameter and skip parameters without a gradient, so the count is tracked per
     tensor (`_count`) and passed to the kernel per tensor.  State mirrors the reference's exactly: a parameter has a
@@ -111,11 +74,9 @@ class _FusedPerTensor(torch.optim.Optimizer):
     _buffers: tuple          # state keys of the flat buffers, in snb_optim_step's argument order
     _has_step: bool = True   # the state carries the reference's per-parameter `step`
 
-    def __init__(self, models: Iterable[NeRF], defaults: dict, precision: Optional[str]):
-        self.models: List[NeRF] = list(models)
-        if not self.models or not all(isinstance(m, NeRF) for m in self.models):
-            raise TypeError(f"{type(self).__name__} steps sinnerf_b200.NeRF models (pass the modules, not their parameters)")
-        super().__init__([p for m in self.models for p in m._param_list()], defaults)
+    def __init__(self, models: Iterable, defaults: dict, precision: Optional[str]):
+        self.models, self._disc = _check_modules(models, type(self).__name__)
+        super().__init__([p for m in self.models for p in _params(m)], defaults)
         self._precision = precision
         self._flat = []          # per model: the flat state buffers, in _buffers order
         self._views = {}         # parameter -> {state key: view of its slice of the flat buffer}
@@ -125,23 +86,28 @@ class _FusedPerTensor(torch.optim.Optimizer):
         if self._flat:
             return
         for m in self.models:
-            ps = m._param_list()
+            ps = _params(m)
             _lib.require_device(ps[0], type(self).__name__)
-            bufs = [torch.zeros(_lib.PARAM_FLOATS, device=ps[0].device, dtype=torch.float32) for _ in self._buffers]
+            total = sum(p.numel() for p in ps)
+            bufs = [torch.zeros(total, device=ps[0].device, dtype=torch.float32) for _ in self._buffers]
             off = 0
             for p in ps:
                 n = p.numel()
                 self._views[p] = {k: b[off:off + n].view_as(p) for k, b in zip(self._buffers, bufs)}
                 self._count[p] = 0
                 off += n
-            assert off == _lib.PARAM_FLOATS
+            assert self._disc or off == _lib.PARAM_FLOATS
             self._flat.append(bufs)
+
+    def _step_value(self, n: int):
+        """The state's `step` entry after n updates, in the type the replaced optimiser keeps it."""
+        return n
 
     def _publish(self):
         self.state.clear()
         for p, n in self._count.items():
             if n > 0:
-                self.state[p] = dict(self._views[p], **({"step": n} if self._has_step else {}))
+                self.state[p] = dict(self._views[p], **({"step": self._step_value(n)} if self._has_step else {}))
 
     def load_state_dict(self, state_dict):
         """Values are copied INTO the flat buffers (the kernel addresses them by offset); a parameter without state
@@ -179,24 +145,117 @@ class _FusedPerTensor(torch.optim.Optimizer):
         args = self._args(group)
         adv = self._advances(group)
         for m, bufs in zip(self.models, self._flat):
-            prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
-            ps = m._param_list()
+            ps = _params(m)
             dev = ps[0].device
+            _check_tensors(ps, type(self).__name__)
             for p in ps:
-                if p.dtype != torch.float32 or not p.is_contiguous() or (p.grad is not None and not p.grad.is_contiguous()):
-                    raise ValueError(f"{type(self).__name__}: parameters and gradients must be contiguous fp32 CUDA tensors")
-            for i, p in enumerate(ps):
                 if p.grad is not None and adv:
                     self._count[p] += 1
-                args.step[i] = self._count[p]
-            image = m.packed_image_buffer(prec)
-            parr = (C.c_void_p * 24)(*[p.data_ptr() for p in ps])
-            garr = (C.c_void_p * 24)(*[(p.grad.data_ptr() if p.grad is not None else None) for p in ps])
+            parr = (C.c_void_p * len(ps))(*[p.data_ptr() for p in ps])
+            garr = (C.c_void_p * len(ps))(*[(p.grad.data_ptr() if p.grad is not None else None) for p in ps])
             st = [_lib.ptr(b) for b in bufs] + [None] * (3 - len(bufs))
             with torch.cuda.device(dev):
+                if self._disc:
+                    _lib.check(lib.snb_optim_step_tensors(len(ps), parr, garr,
+                                                          (C.c_int64 * len(ps))(*[p.numel() for p in ps]),
+                                                          (C.c_int * len(ps))(*[self._count[p] for p in ps]), *st,
+                                                          C.byref(args), _lib.stream_ptr(dev)), "snb_optim_step_tensors")
+                    continue
+                prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
+                for i, p in enumerate(ps):
+                    args.step[i] = self._count[p]
+                image = m.packed_image_buffer(prec)
                 _lib.check(lib.snb_optim_step(parr, garr, *st, C.byref(args), prec, int(m.use_new_activation),
                                               _lib.ptr(image), _lib.stream_ptr(dev)), "snb_optim_step")
         self._publish()
+        return loss
+
+
+class FusedAdam(_FusedPerTensor):
+    """torch.optim.Adam(lr, betas, eps, weight_decay), amsgrad off.  NeRF models: one step count for the optimiser and
+    state for every tensor from the first step, the 24-tensor kernel and the re-pack (snb_adam_step).  Discriminator
+    modules: torch's per-parameter `step` (a tensor, as torch keeps it) and lazily created state (the per-tensor body
+    above, rule SNB_OPTIM_ADAM)."""
+    _rule = _lib.OPTIM_ADAM
+    _buffers = ("exp_avg", "exp_avg_sq")
+
+    def __init__(self, models: Iterable, lr: float = 5e-4, betas=(0.9, 0.999), eps: float = 1e-8,
+                 weight_decay: float = 0.0, precision: Optional[str] = None):
+        super().__init__(models, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), precision)
+        self._steps = 0          # NeRF models: updates applied so far
+
+    def _step_value(self, n):
+        return torch.tensor(float(n))
+
+    def _args(self, group):
+        return _lib.SnbOptimArgs(rule=self._rule, lr=float(group["lr"]), weight_decay=float(group["weight_decay"]),
+                                 beta1=float(group["betas"][0]), beta2=float(group["betas"][1]), eps=float(group["eps"]),
+                                 k=1)
+
+    def _ensure_state(self):
+        if self._disc:
+            return super()._ensure_state()
+        if self._flat:
+            return
+        for m in self.models:
+            ps = m._param_list()
+            dev = ps[0].device
+            _lib.require_device(ps[0], "FusedAdam")
+            ea = torch.zeros(_lib.PARAM_FLOATS, device=dev, dtype=torch.float32)
+            es = torch.zeros(_lib.PARAM_FLOATS, device=dev, dtype=torch.float32)
+            off = 0
+            for p in ps:
+                n = p.numel()
+                self.state[p] = {"step": torch.tensor(float(self._steps)), "exp_avg": ea[off:off + n].view_as(p),
+                                 "exp_avg_sq": es[off:off + n].view_as(p)}
+                off += n
+            assert off == _lib.PARAM_FLOATS
+            self._flat.append((ea, es))
+
+    def load_state_dict(self, state_dict):
+        """Values are copied INTO the flat buffers (the kernel addresses them by offset)."""
+        if self._disc:
+            return super().load_state_dict(state_dict)
+        self._ensure_state()
+        views = {id(p): dict(st) for p, st in self.state.items()}
+        torch.optim.Optimizer.load_state_dict(self, state_dict)
+        step = 0
+        for p, st in self.state.items():
+            keep = views[id(p)]
+            for k in ("exp_avg", "exp_avg_sq"):
+                keep[k].copy_(st[k])
+                st[k] = keep[k]
+            step = max(step, int(float(st.get("step", 0))))
+        self._steps = step
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        if self._disc:
+            return super().step(closure)
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        self._ensure_state()
+        lib = _lib.load()
+        g = self.param_groups[0]
+        self._steps += 1
+        args = _lib.SnbAdamArgs(float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]),
+                                float(g["weight_decay"]), self._steps)
+        for m, (ea, es) in zip(self.models, self._flat):
+            prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
+            ps = m._param_list()
+            dev = ps[0].device
+            _check_tensors(ps, "FusedAdam")
+            image = m.packed_image_buffer(prec)
+            parr = (C.c_void_p * 24)(*[p.data_ptr() for p in ps])
+            garr = (C.c_void_p * 24)(*[(p.grad.data_ptr() if p.grad is not None else None) for p in ps])
+            with torch.cuda.device(dev):
+                _lib.check(lib.snb_adam_step(parr, garr, _lib.ptr(ea), _lib.ptr(es), C.byref(args), prec,
+                                             int(m.use_new_activation), _lib.ptr(image), _lib.stream_ptr(dev)),
+                           "snb_adam_step")
+        for st in self.state.values():
+            st["step"] = torch.tensor(float(self._steps))
         return loss
 
 
@@ -208,7 +267,7 @@ class FusedSGD(_FusedPerTensor):
     _buffers = ("momentum_buffer",)
     _has_step = False
 
-    def __init__(self, models: Iterable[NeRF], lr: float, momentum: float = 0.0, weight_decay: float = 0.0,
+    def __init__(self, models: Iterable, lr: float, momentum: float = 0.0, weight_decay: float = 0.0,
                  precision: Optional[str] = None):
         super().__init__(models, dict(lr=lr, momentum=momentum, dampening=0.0, weight_decay=weight_decay,
                                       nesterov=False), precision)
@@ -230,7 +289,7 @@ class FusedRAdam(_FusedPerTensor):
     _rule = _lib.OPTIM_RADAM
     _buffers = ("exp_avg", "exp_avg_sq")
 
-    def __init__(self, models: Iterable[NeRF], lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
+    def __init__(self, models: Iterable, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, precision: Optional[str] = None):
         super().__init__(models, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
                                       buffer=[[None, None, None] for _ in range(10)]), precision)
@@ -248,7 +307,7 @@ class FusedRanger(_FusedPerTensor):
     _rule = _lib.OPTIM_RANGER
     _buffers = ("exp_avg", "exp_avg_sq", "slow_buffer")
 
-    def __init__(self, models: Iterable[NeRF], lr: float = 1e-3, alpha: float = 0.5, k: int = 6,
+    def __init__(self, models: Iterable, lr: float = 1e-3, alpha: float = 0.5, k: int = 6,
                  N_sma_threshhold: float = 5, betas=(0.95, 0.999), eps: float = 1e-5, weight_decay: float = 0.0,
                  precision: Optional[str] = None):
         super().__init__(models, dict(lr=lr, alpha=alpha, k=k, step_counter=0, betas=betas,
@@ -263,7 +322,8 @@ class FusedRanger(_FusedPerTensor):
 
 def get_optimizer(hparams, models, rate=1):
     """Drop-in for reference utils/__init__.py:10-31: `hparams.optimizer` sgd / adam / radam / ranger with the
-    reference's arguments (lr * rate, eps = 1e-8, momentum for sgd, weight_decay), each fused."""
+    reference's arguments (lr * rate, eps = 1e-8, momentum for sgd, weight_decay), each fused.  `models` is the NeRF
+    models (`self.models`) or the discriminator (`[self.D]`, rate=0.2); any other module raises TypeError."""
     lr, wd = hparams.lr * rate, hparams.weight_decay
     if hparams.optimizer == "sgd":
         return FusedSGD(models, lr=lr, momentum=hparams.momentum, weight_decay=wd)
