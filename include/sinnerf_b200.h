@@ -404,7 +404,11 @@ typedef struct SnbDiscAug {
   const int64_t* cutout_y;   /* (n,) torch.randint offset along the rows */
   const int64_t* cutout_x;   /* (n,) ... along the columns */
 } SnbDiscAug;
-/* 0 for a shape the branch cannot run (a convolution with an empty output, an InstanceNorm over one element) */
+/* 0 for a shape the branch cannot run (a convolution with an empty output, an InstanceNorm over one element) or
+ * that is too large: n times any layer's output pixels above 65535 x 64 = 4194240 (the rows of that layer's input
+ * gradient GEMM; the first layer has the most: n oh ow of (h / 2) x (w / 2) roughly, so at most 1023 images of
+ * 128 x 128 or 4095 of 64 x 64), or n times a layer's output pixels times 16 in-channels at 2^31 or more.  The
+ * forward and backward refuse the same shapes. */
 size_t snb_disc_workspace_bytes(int imsize, int n, int height, int width, int save);
 int snb_disc_forward(int imsize, int precision, int training, const float* const* weights, float* const* weight_u,
                      float* const* weight_v, const float* input, const int64_t* strides, int n, int height, int width,

@@ -19,9 +19,11 @@
 // [2^14, 2^15)) before the chain, each layer's output gradient is rescaled the same way after its fold, the GEMMs
 // read a copy of each weight scaled likewise, and normalised activations are scaled on their way into im2col; the
 // exponents are undone in the GEMMs' alpha and in the final gradients.
-// Every factor is a power of two, so this is exact, and it keeps the fp16 hi / lo operand words out of their
-// subnormal range whatever the loss weight.  Every reduction runs in a fixed order: two identical calls give the same
-// bits.
+// Every factor is a power of two, and it keeps the fp16 hi / lo operand words out of their subnormal range whatever
+// the loss weight.  The gradient exponents are carried as integers and applied once, with ldexpf, as each final
+// gradient is written: the scaling is exact wherever that gradient is a normal float, and below that it is rounded
+// once (never flushed to zero by an intermediate factor).  Every reduction runs in a fixed order: two identical calls
+// give the same bits.
 #include "common.cuh"
 #include "tc_gemm.cuh"
 
@@ -72,6 +74,10 @@ int net_of(const char* who, int imsize, int n, int h, int w, Net& net) {
     SNB_REQUIRE(!y.in_norm || y.P() > 1,
                 "%s: a %d x %d image leaves one spatial element for layer %d's InstanceNorm", who, h, w, i);
     SNB_REQUIRE((long long)n * y.P() * y.K() < (1ll << 31), "%s: batch %d of %d x %d images is too large", who, n, h, w);
+    // the dgrad GEMM tiles layer i's n P rows 64 to a block along grid.y
+    SNB_REQUIRE((long long)n * y.P() <= kMaxGemmRows,
+                "%s: batch %d of %d x %d images gives layer %d %lld rows (n x %d x %d output pixels), more than its input "
+                "gradient GEMM's %lld", who, n, h, w, i, (long long)n * y.P(), y.hout, y.wout, kMaxGemmRows);
     H = y.hout; W = y.wout;
   }
   return SNB_OK;
@@ -80,7 +86,8 @@ int net_of(const char* who, int imsize, int n, int h, int w, Net& net) {
 // ------------------------------------------------------------------ workspace
 long long al64(long long x) { return (x + 63) & ~63ll; }
 struct DiscWs {
-  float *sigma, *inv_sigma, *alpha, *wscale, *aug, *ginv, *dot;
+  float *sigma, *inv_sigma, *alpha, *wscale, *aug, *dot;
+  int* gexp;                      // per layer: the exponent that undoes the scaling of its output gradient
   float *u[kMaxLayers], *v[kMaxLayers], *t[kMaxLayers], *s[kMaxLayers], *rmax[kMaxLayers], *part[kMaxLayers];
   float* ws[kMaxLayers];          // 2^e W_orig, its largest element in [2^14, 2^15)
   float *col[kMaxLayers], *y[kMaxLayers], *mean[kMaxLayers], *rstd[kMaxLayers];
@@ -93,7 +100,7 @@ DiscWs disc_ws(void* base, const Net& N, int save) {
   long long off = 0;
   auto take = [&](long long floats) { float* p = b == nullptr ? nullptr : b + off; off = al64(off + floats); return p; };
   W.sigma = take(kMaxLayers); W.inv_sigma = take(kMaxLayers); W.alpha = take(kMaxLayers); W.wscale = take(kMaxLayers);
-  W.dot = take(kMaxLayers); W.ginv = take(kMaxLayers);
+  W.dot = take(kMaxLayers); W.gexp = reinterpret_cast<int*>(take(kMaxLayers));
   W.aug = take((long long)kAugFloats * N.n);
   long long dy_max = 0, dcol_max = 0;
   for (int i = 0; i < N.n_layers; ++i) {
@@ -409,27 +416,28 @@ __global__ void disc_fold_kernel(const FoldArgs a) {
 }
 
 // ------------------------------------------------------------------ gradient scale and DiffAugment backward
-// dy = g 2^k with the largest |dy| in [2^14, 2^15) (dy may be g); inv_out = inv_in 2^-k (inv_in null: 1).  Applied to the
+// dy = g 2^k with the largest |dy| in [2^14, 2^15) (dy may be g); e_out = e_in - k (e_in null: 0).  Applied to the
 // upstream gradient and again to each layer's output gradient, so that no GEMM operand drifts into fp16's
-// subnormal range along the chain; every factor is a power of two, so the scaling is exact.
-__global__ void disc_grad_scale_kernel(const float* g, long long m, float* dy, const float* __restrict__ inv_in,
-                                       float* __restrict__ inv_out) {
+// subnormal range along the chain.  The exponent stays an integer: as a float factor 2^e_out it would underflow to 0
+// for an upstream below 2^-135 or a chain that shrinks the gradients far enough.
+__global__ void disc_grad_scale_kernel(const float* g, long long m, float* dy, const int* __restrict__ e_in,
+                                       int* __restrict__ e_out) {
   __shared__ float red[32];
   float mx = 0.f;
   for (long long i = threadIdx.x; i < m; i += blockDim.x) mx = fmaxf(mx, fabsf(g[i]));
   const int k = pow2_exponent(block_max(mx, red));
   for (long long i = threadIdx.x; i < m; i += blockDim.x) dy[i] = ldexpf(g[i], k);
-  if (threadIdx.x == 0) *inv_out = ldexpf(inv_in != nullptr ? *inv_in : 1.f, -k);
+  if (threadIdx.x == 0) *e_out = (e_in != nullptr ? *e_in : 0) - k;
 }
 
 // one block per image: dx (3, n, h w) -> the input gradient through d_strides, unscaled
 __global__ void disc_aug_bwd_kernel(const float* __restrict__ dx, const float* __restrict__ aug, int n, int h, int w,
-                                    const float* __restrict__ ginv, float* __restrict__ out, long long s_b,
+                                    const int* __restrict__ gexp, float* __restrict__ out, long long s_b,
                                     long long s_c, long long s_y, long long s_x) {
   __shared__ float red[32];
   const int b = blockIdx.x, P = h * w;
   const float* q = aug + (long long)kAugFloats * b;
-  const float inv = *ginv;
+  const int e = *gexp;
   const bool on = q[0] != 0.f;
   float S = 0.f;
   if (on) {
@@ -449,7 +457,7 @@ __global__ void disc_aug_bwd_kernel(const float* __restrict__ dx, const float* _
       const float m = (g[0] + g[1] + g[2]) / 3.f;
       for (int c = 0; c < 3; ++c) g[c] = sat * g[c] + (1.f - sat) * m;
     }
-    for (int c = 0; c < 3; ++c) out[b * s_b + c * s_c + y * s_y + x * s_x] = g[c] * inv;
+    for (int c = 0; c < 3; ++c) out[b * s_b + c * s_c + y * s_y + x * s_x] = ldexpf(g[c], e);
   }
 }
 
@@ -460,7 +468,8 @@ struct FixArgs {
   const float *u[kMaxLayers], *v[kMaxLayers];
   float* part[kMaxLayers];
   int rows[kMaxLayers], cols[kMaxLayers];
-  const float *inv_sigma, *ginv;
+  const float* inv_sigma;
+  const int* gexp;
 };
 
 // part[r] = <dW[r], W[r]>
@@ -475,7 +484,7 @@ __global__ void disc_sn_dot_kernel(const FixArgs a) {
   if (threadIdx.x == 0) a.part[l][r] = acc;
 }
 
-// dW = (dW / sigma - (<dW, W> / sigma^2) u v^T) ginv; every block sums part[] in the same order
+// dW = (dW / sigma - (<dW, W> / sigma^2) u v^T) 2^gexp; every block sums part[] in the same order
 __global__ void disc_sn_fix_kernel(const FixArgs a) {
   __shared__ float red[32];
   const int l = blockIdx.y;
@@ -489,7 +498,7 @@ __global__ void disc_sn_fix_kernel(const FixArgs a) {
   if (i >= n) return;
   const float is = a.inv_sigma[l], c = d * is * is;
   const int r = (int)(i / a.cols[l]), k = (int)(i % a.cols[l]);
-  a.dW[l][i] = (a.dW[l][i] * is - c * a.u[l][r] * a.v[l][k]) * a.ginv[l];
+  a.dW[l][i] = ldexpf(a.dW[l][i] * is - c * a.u[l][r] * a.v[l][k], a.gexp[l]);
 }
 
 // ------------------------------------------------------------------ host
@@ -579,7 +588,7 @@ int disc_backward_impl(const Net& N, const float* const* W, const float* d_out, 
   const Layer& last = N.l[L - 1];
   float* dy = ws.dy0;
   float* dy_next = ws.dy1;
-  disc_grad_scale_kernel<<<1, 1024, 0, st>>>(d_out, (long long)N.n * last.P(), dy, nullptr, ws.ginv + L - 1);
+  disc_grad_scale_kernel<<<1, 1024, 0, st>>>(d_out, (long long)N.n * last.P(), dy, nullptr, ws.gexp + L - 1);
   DISC_TRY(check_launch("disc_grad_scale_kernel"));
   // lowest layer whose input gradient is needed
   int stop = d_input != nullptr ? 0 : L;
@@ -616,14 +625,14 @@ int disc_backward_impl(const Net& N, const float* const* W, const float* d_out, 
     disc_fold_kernel<<<y.cin * N.n, 256, 0, st>>>(f);
     DISC_TRY(check_launch("disc_fold_kernel"));
     if (i > 0) {
-      disc_grad_scale_kernel<<<1, 1024, 0, st>>>(dy_next, (long long)y.cin * N.n * y.hin * y.win, dy_next, ws.ginv + i,
-                                                 ws.ginv + i - 1);
+      disc_grad_scale_kernel<<<1, 1024, 0, st>>>(dy_next, (long long)y.cin * N.n * y.hin * y.win, dy_next, ws.gexp + i,
+                                                 ws.gexp + i - 1);
       DISC_TRY(check_launch("disc_grad_scale_kernel"));
     }
     float* tmp = dy; dy = dy_next; dy_next = tmp;
   }
   if (d_input != nullptr) {
-    disc_aug_bwd_kernel<<<N.n, 256, 0, st>>>(ws.dx, ws.aug, N.n, N.h, N.w, ws.ginv, d_input, ds[0], ds[1], ds[2], ds[3]);
+    disc_aug_bwd_kernel<<<N.n, 256, 0, st>>>(ws.dx, ws.aug, N.n, N.h, N.w, ws.gexp, d_input, ds[0], ds[1], ds[2], ds[3]);
     DISC_TRY(check_launch("disc_aug_bwd_kernel"));
   }
   FixArgs a{};
@@ -637,7 +646,7 @@ int disc_backward_impl(const Net& N, const float* const* W, const float* d_out, 
       most = most > N.l[i].cout * N.l[i].K() ? most : N.l[i].cout * N.l[i].K();
     }
   }
-  a.inv_sigma = ws.inv_sigma; a.ginv = ws.ginv;
+  a.inv_sigma = ws.inv_sigma; a.gexp = ws.gexp;
   if (any) {
     disc_sn_dot_kernel<<<dim3(512, L), 256, 0, st>>>(a);
     DISC_TRY(check_launch("disc_sn_dot_kernel"));

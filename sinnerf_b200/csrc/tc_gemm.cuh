@@ -27,7 +27,12 @@ int mode_of(int precision) {
   }
 }
 
-__device__ __forceinline__ float clamp_f16(float x) { return fminf(fmaxf(x, -65504.f), 65504.f); }
+// to fp16's finite range; NaN stays NaN (fminf / fmaxf would return the bound)
+__device__ __forceinline__ float clamp_f16(float x) {
+  float y;
+  asm("max.NaN.f32 %0, %1, 0fC77FE000;\n\tmin.NaN.f32 %0, %0, 0f477FE000;" : "=f"(y) : "f"(x));
+  return y;
+}
 
 // two fp32 values -> the packed 16-bit pair(s) of the mode (lo only in split mode)
 template <int kMode>
@@ -71,6 +76,7 @@ struct Gemm {
 };
 
 constexpr int kTile = 64, kChunk = 64, kGemmThreads = 128;
+constexpr long long kMaxGemmRows = 65535ll * kTile;   // M tiles along grid.y, at most 65535 of them
 constexpr int kPlaneBytes = kTile * kChunk * 2;   // one 64 x 64 16-bit operand tile
 
 __device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
@@ -235,6 +241,9 @@ int run_gemm(Gemm g, int nz, cudaStream_t st) {
   if (g.M <= 0 || g.N <= 0 || nz <= 0) return SNB_OK;
   if (g.nz2 <= 0) g.nz2 = 1;
   g.a_vec = g.a_k == 1 && aligned16(g.A) && g.a_m % 4 == 0 && g.a_z1 % 4 == 0 && g.a_z2 % 4 == 0;
+  if (g.M > kMaxGemmRows || nz > 65535)
+    return fail(SNB_ERR_INVALID, "vit_gemm_kernel: %d x %d x %d GEMM over %d matrices exceeds the launch grid (at most "
+                "%lld rows, 65535 matrices)", g.M, g.N, g.K, nz, kMaxGemmRows);
   const dim3 grid((g.N + kTile - 1) / kTile, (g.M + kTile - 1) / kTile, nz);
   if (g.Bf != nullptr) {
     g.b_vec = g.b_k == 1 && aligned16(g.Bf) && g.b_n % 4 == 0 && g.b_z1 % 4 == 0 && g.b_z2 % 4 == 0;
