@@ -310,7 +310,8 @@ int snb_depth_smooth_backward(const float* idepth, const int64_t* idepth_strides
  * of 5, depthwise correlation with the 11x11 Gaussian window (sigma 1.5) of img1, img2, img1^2, img2^2, img1 img2, and
  * mean clamp((1 - ssim) / 2, 0, 1), C1 = (0.01 max_val)^2, C2 = (0.03 max_val)^2.  window_size other than 11:
  * SNB_ERR_UNSUPPORTED.  The window sums and the SSIM expression are evaluated in fp64 (see DESIGN.md section 4).
- * coef: NULL (no backward), or a device buffer of 3 B C H W doubles the forward fills with the per-pixel
+ * The clamp keeps a NaN, as torch.clamp does: a NaN in either image makes the loss NaN.  C1 and C2 are formed from
+ * max_val as passed, a float32.  coef: NULL (no backward), or a device buffer of 3 B C H W doubles the forward fills with the per-pixel
  * coefficient maps snb_ssim_loss_backward reads.  -> loss (1 float) */
 int snb_ssim_loss_forward(const float* img1, const int64_t* img1_strides, const float* img2,
                           const int64_t* img2_strides, int64_t batch, int channels, int height, int width,

@@ -245,7 +245,8 @@ __global__ void __launch_bounds__(kThreads) ssim_fwd_kernel(SsimArgs a, Taps tap
       const double den = B1 * B2 + a.eps;
       const double ssim = A1 * A2 / den;
       const double u = (1.0 - ssim) * 0.5;
-      lsum += (float)fmin(fmax(u, 0.0), 1.0);
+      // torch.clamp keeps a NaN, where fmax(NaN, 0) would return 0: a NaN in either image makes the loss NaN
+      lsum += (float)(isnan(u) ? u : fmin(fmax(u, 0.0), 1.0));
       if (coef != nullptr) {
         // dL/dssim for the mean of clamp(u, 0, 1); torch.clamp passes the gradient for min <= u <= max
         const double gs = (u >= 0.0 && u <= 1.0) ? -0.5 * a.inv_n : 0.0;
