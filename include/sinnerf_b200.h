@@ -489,6 +489,43 @@ int snb_optim_step_tensors(int n, float* const* params, const float* const* grad
                            const int* step, float* exp_avg, float* exp_avg_sq, float* slow_buffer,
                            const SnbOptimArgs* args, void* stream);
 
+/* GradScaler-native forms of the three steps above (torch's `_step_supports_amp_scaling` contract): the gradients
+ * arrive multiplied by a loss scale, and GradScaler's scale and found_inf stay on the device, so the host never waits
+ * for them.  Same arguments as the plain forms, except that grads are written (the unscaled values are stored back)
+ * and the update counts come from `amp` (args->step is not read).  Each gradient element is unscaled exactly as
+ * GradScaler.unscale_ does it: inv = (float)(1 / (double)*scale), g * inv unless inv == 1.  When *found_inf != 0 the
+ * step is skipped: the gradients are still unscaled, but parameters, state buffers, counts, the packed image and its
+ * checksum keep their values (the image header's dirty flag is cleared; it is scratch every refresh recomputes).
+ * Otherwise the update is the plain form's, bit for bit.
+ *   scale: device float, or NULL = the gradients are not scaled.  found_inf: device float, or NULL = never skip.
+ *   count_in / count_out: device arrays of update counts (1 for snb_adam_step_amp, one per tensor for the others),
+ *     before and after the step; they must not overlap.  A tensor's count advances on a taken step when it has a
+ *     gradient (snb_optim_*: SGD only with momentum); snb_adam_step_amp's single count advances on every taken step.
+ *   base: HOST array, per count: the count the tensor reaches if this step is taken and every earlier step whose
+ *     outcome the host has not read back was skipped.  The step-dependent scalars are formed on the host, in double as
+ *     in the plain forms, for the SNB_OPTIM_WINDOW counts base .. base + SNB_OPTIM_WINDOW - 1, and the kernel picks
+ *     the one at count_in + 1.  The caller guarantees base <= count_in + 1 < base + SNB_OPTIM_WINDOW wherever the
+ *     count advances, reading the counts back (without blocking, a step or more late) to keep the window current.
+ * SNB_ERR_INVALID as for the plain forms, and for a null amp or count array, overlapping count arrays, and base < 1
+ * where a count advances. */
+#define SNB_OPTIM_WINDOW 8
+typedef struct SnbAmpStep {
+  const float* scale;
+  const float* found_inf;
+  const int* count_in;
+  int* count_out;
+  int base[SNB_OPTIM_MAX_TENSORS];
+} SnbAmpStep;
+int snb_adam_step_amp(float* const* params, float* const* grads, float* exp_avg, float* exp_avg_sq,
+                      const SnbAdamArgs* args, const SnbAmpStep* amp, int precision, int new_activation, void* packed,
+                      void* stream);
+int snb_optim_step_amp(float* const* params, float* const* grads, float* exp_avg, float* exp_avg_sq,
+                       float* slow_buffer, const SnbOptimArgs* args, const SnbAmpStep* amp, int precision,
+                       int new_activation, void* packed, void* stream);
+int snb_optim_step_tensors_amp(int n, float* const* params, float* const* grads, const int64_t* numel,
+                               float* exp_avg, float* exp_avg_sq, float* slow_buffer, const SnbOptimArgs* args,
+                               const SnbAmpStep* amp, void* stream);
+
 /* ---- whole path -------------------------------------------------------------------- */
 typedef struct SnbRenderArgs {
   const float* rays;        /* (N,8)                                                    */

@@ -63,6 +63,14 @@ class SnbOptimArgs(C.Structure):
                 ("alpha", C.c_double), ("k", C.c_int), ("step", C.c_int * 24)]
 
 
+OPTIM_WINDOW = 8   # SNB_OPTIM_WINDOW
+
+
+class SnbAmpStep(C.Structure):
+    _fields_ = [("scale", c_f), ("found_inf", c_f), ("count_in", c_f), ("count_out", c_f),
+                ("base", C.c_int * OPTIM_MAX_TENSORS)]
+
+
 class SnbDiscAug(C.Structure):
     _fields_ = [("brightness", c_f), ("saturation", c_f), ("contrast", c_f), ("cutout_y", c_f), ("cutout_x", c_f)]
 
@@ -112,6 +120,13 @@ SIGNATURES = {
                                  C.c_int, C.c_int, c_f, c_f]),
     "snb_optim_step_tensors": (C.c_int, [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int), c_f, c_f, c_f, C.POINTER(SnbOptimArgs), c_f]),
+    "snb_adam_step_amp": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, C.POINTER(SnbAdamArgs),
+                                    C.POINTER(SnbAmpStep), C.c_int, C.c_int, c_f, c_f]),
+    "snb_optim_step_amp": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, c_f,
+                                     C.POINTER(SnbOptimArgs), C.POINTER(SnbAmpStep), C.c_int, C.c_int, c_f, c_f]),
+    "snb_optim_step_tensors_amp": (C.c_int, [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                             C.POINTER(C.c_int64), c_f, c_f, c_f, C.POINTER(SnbOptimArgs),
+                                             C.POINTER(SnbAmpStep), c_f]),
     "snb_field_backward": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, c_f, c_f, c_f, c_f, c_f,
                                      c_f, C.c_int64, c_f, c_f, c_f, c_f, c_f, c_f]),
     "snb_field_forward_train_sigma": (C.c_int, [c_f, C.c_int, c_f, c_f, C.c_int64, C.c_int, c_f, c_f, c_f, c_f]),

@@ -74,6 +74,12 @@ int optim_step_pack(float* const*, const float* const*, float*, float*, float*, 
                     cudaStream_t);
 int optim_step_tensors(int, float* const*, const float* const*, const int64_t*, const int*, float*, float*, float*,
                        const SnbOptimArgs&, cudaStream_t);
+int adam_step_pack_amp(float* const*, float* const*, float*, float*, const SnbAdamArgs&, const SnbAmpStep&, int, int,
+                       void*, cudaStream_t);
+int optim_step_pack_amp(float* const*, float* const*, float*, float*, float*, const SnbOptimArgs&, const SnbAmpStep&,
+                        int, int, void*, cudaStream_t);
+int optim_step_tensors_amp(int, float* const*, float* const*, const int64_t*, float*, float*, float*,
+                           const SnbOptimArgs&, const SnbAmpStep&, cudaStream_t);
 // tensor-core modes (field_tc.cu)
 size_t tc_packed_bytes(int precision);
 int field_forward_tc(const void*, int, const float*, const float*, int64_t, int, int, float*, cudaStream_t);
@@ -459,52 +465,52 @@ int snb_field_backward16_sigma(const float* const* params, float* const* grads, 
                                 reinterpret_cast<cudaStream_t>(stream));
 }
 
-int snb_adam_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
-                  const SnbAdamArgs* args, int precision, int new_activation, void* packed, void* stream) {
-  SNB_REQUIRE(params && grads && exp_avg && exp_avg_sq && args, "snb_adam_step: null pointer");
-  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) SNB_REQUIRE(params[i] != nullptr, "snb_adam_step: parameter tensor %d is null", i);
-  SNB_REQUIRE(args->step >= 1, "snb_adam_step: step counts from 1 (got %d)", args->step);
+// Argument checks shared by the plain and GradScaler-native (_amp) forms of the three optimiser steps.  `step` is the
+// plain form's count (snb_adam_step: one; the others: per tensor), or the _amp form's `base`, which the same rules bound.
+static int check_adam_step(const char* who, float* const* params, const void* grads, const float* exp_avg,
+                           const float* exp_avg_sq, const SnbAdamArgs* args, const int* step, int precision,
+                           const void* packed) {
+  SNB_REQUIRE(params && grads && exp_avg && exp_avg_sq && args && step, "%s: null pointer", who);
+  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) SNB_REQUIRE(params[i] != nullptr, "%s: parameter tensor %d is null", who, i);
+  SNB_REQUIRE(*step >= 1, "%s: step counts from 1 (got %d)", who, *step);
   SNB_REQUIRE(args->lr >= 0. && args->eps >= 0. && args->beta1 >= 0. && args->beta1 < 1. && args->beta2 >= 0. &&
                   args->beta2 < 1. && args->weight_decay >= 0.,
-              "snb_adam_step: invalid hyper-parameters");
-  SNB_REQUIRE(packed == nullptr || aligned16(packed), "snb_adam_step: packed image must be 16-byte aligned");
+              "%s: invalid hyper-parameters", who);
+  SNB_REQUIRE(packed == nullptr || aligned16(packed), "%s: packed image must be 16-byte aligned", who);
   if (packed != nullptr)
     if (int rc = check_precision(precision)) return rc;
   static_assert(SNB_PARAM_FLOATS == 593408 + 2436, "parameter count");
-  return adam_step_pack(params, grads, exp_avg, exp_avg_sq, *args, precision, new_activation, packed,
-                        reinterpret_cast<cudaStream_t>(stream));
+  return SNB_OK;
 }
 
-int snb_optim_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
-                   float* slow_buffer, const SnbOptimArgs* args, int precision, int new_activation, void* packed,
-                   void* stream) {
-  SNB_REQUIRE(params && grads && args, "snb_optim_step: null pointer");
+static int check_optim_step(const char* who, float* const* params, const void* const* grads, const float* exp_avg,
+                            const float* exp_avg_sq, const float* slow_buffer, const SnbOptimArgs* args,
+                            const int* step, int precision, const void* packed) {
+  SNB_REQUIRE(params && grads && args, "%s: null pointer", who);
   const int rule = args->rule;
   SNB_REQUIRE(rule == SNB_OPTIM_SGD || rule == SNB_OPTIM_RADAM || rule == SNB_OPTIM_RANGER,
-              "snb_optim_step: unknown rule %d", rule);
+              "%s: unknown rule %d", who, rule);
   SNB_REQUIRE(exp_avg != nullptr && (rule == SNB_OPTIM_SGD || exp_avg_sq != nullptr) &&
                   (rule != SNB_OPTIM_RANGER || slow_buffer != nullptr),
-              "snb_optim_step: null state buffer");
+              "%s: null state buffer", who);
   for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) {
-    SNB_REQUIRE(params[i] != nullptr, "snb_optim_step: parameter tensor %d is null", i);
-    SNB_REQUIRE(grads[i] == nullptr || args->step[i] >= 1 || (rule == SNB_OPTIM_SGD && args->momentum == 0.),
-                "snb_optim_step: step of tensor %d counts from 1 (got %d)", i, args->step[i]);
+    SNB_REQUIRE(params[i] != nullptr, "%s: parameter tensor %d is null", who, i);
+    SNB_REQUIRE(grads[i] == nullptr || step[i] >= 1 || (rule == SNB_OPTIM_SGD && args->momentum == 0.),
+                "%s: step of tensor %d counts from 1 (got %d)", who, i, step[i]);
   }
   SNB_REQUIRE(args->lr >= 0. && args->weight_decay >= 0. && args->momentum >= 0. && args->eps >= 0. &&
                   args->beta1 >= 0. && args->beta1 < 1. && args->beta2 >= 0. && args->beta2 < 1. &&
                   args->alpha >= 0. && args->alpha <= 1. && args->k >= 1,
-              "snb_optim_step: invalid hyper-parameters");
-  SNB_REQUIRE(packed == nullptr || aligned16(packed), "snb_optim_step: packed image must be 16-byte aligned");
+              "%s: invalid hyper-parameters", who);
+  SNB_REQUIRE(packed == nullptr || aligned16(packed), "%s: packed image must be 16-byte aligned", who);
   if (packed != nullptr)
     if (int rc = check_precision(precision)) return rc;
-  return optim_step_pack(params, grads, exp_avg, exp_avg_sq, slow_buffer, *args, precision, new_activation, packed,
-                         reinterpret_cast<cudaStream_t>(stream));
+  return SNB_OK;
 }
 
-int snb_optim_step_tensors(int n, float* const* params, const float* const* grads, const int64_t* numel,
-                           const int* step, float* exp_avg, float* exp_avg_sq, float* slow_buffer,
-                           const SnbOptimArgs* args, void* stream) {
-  const char* who = "snb_optim_step_tensors";
+static int check_optim_tensors(const char* who, int n, float* const* params, const void* const* grads,
+                               const int64_t* numel, const int* step, const float* exp_avg, const float* exp_avg_sq,
+                               const float* slow_buffer, const SnbOptimArgs* args) {
   SNB_REQUIRE(params && grads && numel && step && args, "%s: null table or args", who);
   SNB_REQUIRE(n >= 1 && n <= SNB_OPTIM_MAX_TENSORS, "%s: needs 1 <= n <= %d tensors (got %d)", who,
               SNB_OPTIM_MAX_TENSORS, n);
@@ -525,8 +531,78 @@ int snb_optim_step_tensors(int n, float* const* params, const float* const* grad
                   args->beta1 >= 0. && args->beta1 < 1. && args->beta2 >= 0. && args->beta2 < 1. &&
                   args->alpha >= 0. && args->alpha <= 1. && args->k >= 1,
               "%s: invalid hyper-parameters", who);
+  return SNB_OK;
+}
+
+// The _amp forms' own arguments: n counts in each of two device arrays that must not overlap.
+static int check_amp(const char* who, const SnbAmpStep* amp, int n) {
+  SNB_REQUIRE(amp != nullptr && amp->count_in != nullptr && amp->count_out != nullptr, "%s: null amp or count array", who);
+  SNB_REQUIRE(amp->count_in + n <= amp->count_out || amp->count_out + n <= amp->count_in,
+              "%s: count_in and count_out overlap", who);
+  return SNB_OK;
+}
+
+int snb_adam_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
+                  const SnbAdamArgs* args, int precision, int new_activation, void* packed, void* stream) {
+  if (int rc = check_adam_step("snb_adam_step", params, grads, exp_avg, exp_avg_sq, args, args ? &args->step : nullptr,
+                               precision, packed))
+    return rc;
+  return adam_step_pack(params, grads, exp_avg, exp_avg_sq, *args, precision, new_activation, packed,
+                        reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_adam_step_amp(float* const* params, float* const* grads, float* exp_avg, float* exp_avg_sq,
+                      const SnbAdamArgs* args, const SnbAmpStep* amp, int precision, int new_activation, void* packed,
+                      void* stream) {
+  const char* who = "snb_adam_step_amp";
+  if (int rc = check_amp(who, amp, 1)) return rc;
+  if (int rc = check_adam_step(who, params, grads, exp_avg, exp_avg_sq, args, amp->base, precision, packed)) return rc;
+  return adam_step_pack_amp(params, grads, exp_avg, exp_avg_sq, *args, *amp, precision, new_activation, packed,
+                            reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_optim_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
+                   float* slow_buffer, const SnbOptimArgs* args, int precision, int new_activation, void* packed,
+                   void* stream) {
+  if (int rc = check_optim_step("snb_optim_step", params, reinterpret_cast<const void* const*>(grads), exp_avg,
+                                exp_avg_sq, slow_buffer, args, args ? args->step : nullptr, precision, packed))
+    return rc;
+  return optim_step_pack(params, grads, exp_avg, exp_avg_sq, slow_buffer, *args, precision, new_activation, packed,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_optim_step_amp(float* const* params, float* const* grads, float* exp_avg, float* exp_avg_sq,
+                       float* slow_buffer, const SnbOptimArgs* args, const SnbAmpStep* amp, int precision,
+                       int new_activation, void* packed, void* stream) {
+  const char* who = "snb_optim_step_amp";
+  if (int rc = check_amp(who, amp, SNB_N_PARAM_TENSORS)) return rc;
+  if (int rc = check_optim_step(who, params, reinterpret_cast<const void* const*>(grads), exp_avg, exp_avg_sq,
+                                slow_buffer, args, amp->base, precision, packed))
+    return rc;
+  return optim_step_pack_amp(params, grads, exp_avg, exp_avg_sq, slow_buffer, *args, *amp, precision, new_activation,
+                             packed, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_optim_step_tensors(int n, float* const* params, const float* const* grads, const int64_t* numel,
+                           const int* step, float* exp_avg, float* exp_avg_sq, float* slow_buffer,
+                           const SnbOptimArgs* args, void* stream) {
+  if (int rc = check_optim_tensors("snb_optim_step_tensors", n, params, reinterpret_cast<const void* const*>(grads),
+                                   numel, step, exp_avg, exp_avg_sq, slow_buffer, args))
+    return rc;
   return optim_step_tensors(n, params, grads, numel, step, exp_avg, exp_avg_sq, slow_buffer, *args,
                             reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_optim_step_tensors_amp(int n, float* const* params, float* const* grads, const int64_t* numel,
+                               float* exp_avg, float* exp_avg_sq, float* slow_buffer, const SnbOptimArgs* args,
+                               const SnbAmpStep* amp, void* stream) {
+  const char* who = "snb_optim_step_tensors_amp";
+  if (int rc = check_amp(who, amp, n < 1 ? 1 : (n > SNB_OPTIM_MAX_TENSORS ? SNB_OPTIM_MAX_TENSORS : n))) return rc;
+  if (int rc = check_optim_tensors(who, n, params, reinterpret_cast<const void* const*>(grads), numel, amp->base,
+                                   exp_avg, exp_avg_sq, slow_buffer, args))
+    return rc;
+  return optim_step_tensors_amp(n, params, grads, numel, exp_avg, exp_avg_sq, slow_buffer, *args, *amp,
+                                reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_depth_smooth_forward(const float* idepth, const int64_t* idepth_strides, const float* image,

@@ -353,4 +353,317 @@ int optim_step_tensors(int n, float* const* params, const float* const* grads, c
   return check_launch("optim_tensors_kernel");
 }
 
+// ---------------------------------------------------------------- GradScaler-native steps (snb_*_amp)
+// The three steps above as torch's GradScaler drives an optimiser that sets _step_supports_amp_scaling: the gradients
+// arrive scaled, with GradScaler's scale and found_inf on the device, and the host does not wait for either.
+//   * Every gradient element is unscaled as GradScaler.unscale_ does it -- inv = (float)(1 / (double)scale), then
+//     g * inv unless inv == 1 (torch's _amp_foreach_non_finite_check_and_unscale_) -- and written back to the
+//     gradient, taken step or not, so .grad ends as GradScaler's own unscale leaves it.  __fmul_rn keeps the product
+//     out of any FMA, so the update sees the value it would read back from memory.
+//   * *found_inf != 0: parameters, state, update counts, checksum and image stay as they are (GradScaler never calls
+//     step() then).  The grid reads the same flag, so the branch is uniform.
+//   * The update counts live on the device: the kernel reads count_in and block 0 writes count_out (a second buffer,
+//     so no block can see a count advanced under it).  The step-dependent scalars are formed on the host, in doubles as
+//     above, for the kOptimWindow counts base .. base + kOptimWindow - 1 a tensor can have reached, and each tensor
+//     picks its entry by count_in + 1 - base.  The caller keeps that index in range (SnbAmpStep in the header).
+constexpr int kOptimWindow = SNB_OPTIM_WINDOW;
+
+struct AmpCtl {
+  const float* scale;        // nullable: the gradients carry no scale
+  const float* found_inf;    // nullable: never skip
+  const int* count_in;
+  int* count_out;
+};
+
+__device__ __forceinline__ float amp_inv_scale(const float* scale) {
+  return scale == nullptr ? 1.f : (float)(1.0 / (double)*scale);
+}
+__device__ __forceinline__ bool amp_skip(const float* found_inf) { return found_inf != nullptr && *found_inf != 0.f; }
+// The unscaled gradient element, written back when the scale changes it.
+__device__ __forceinline__ float amp_unscale(float* g, long long e, float inv) {
+  float gr = g[e];
+  if (inv != 1.f) {
+    gr = __fmul_rn(gr, inv);
+    g[e] = gr;
+  }
+  return gr;
+}
+
+struct AdamWindow {
+  int base;
+  float lr_neg_step[kOptimWindow];
+  float inv_bc2_sqrt[kOptimWindow];
+};
+
+// A skipped step clears header.dirty instead of stamping, so the pack kernels that follow (only_if_dirty) return at
+// once and the image keeps the bytes and checksum it had.  The flag is the pack kernels' scratch: every refresh
+// recomputes it from the checksum before it is read.
+__global__ void __launch_bounds__(256) adam_step_amp_kernel(AdamPtrs a, float* __restrict__ exp_avg,
+                                                            float* __restrict__ exp_avg_sq, float beta1_w, float beta2,
+                                                            float beta2_w, float eps, float weight_decay, AdamWindow win,
+                                                            AmpCtl amp, PackedHeader* hdr) {
+  const bool skip = amp_skip(amp.found_inf);
+  const float inv = amp_inv_scale(amp.scale);
+  const int count = amp.count_in[0];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    amp.count_out[0] = skip ? count : count + 1;
+    if (skip && hdr != nullptr) hdr->dirty = 0;
+  }
+  float lr_neg_step = 0.f, inv_bc2_sqrt = 0.f;
+  if (!skip) {
+    lr_neg_step = win.lr_neg_step[count + 1 - win.base];
+    inv_bc2_sqrt = win.inv_bc2_sqrt[count + 1 - win.base];
+  }
+  unsigned long long h = 0;
+  unsigned long long base = 0;
+  for (int t = 0; t < SNB_N_PARAM_TENSORS; ++t) {
+    const int n = param_numel(t);
+    float* p = a.p[t];
+    float* g = const_cast<float*>(a.g[t]);
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
+      const float gr = g != nullptr ? amp_unscale(g, e, inv) : 0.f;
+      if (skip) continue;
+      float w = p[e];
+      if (g != nullptr) {
+        float m = exp_avg[base + e], v = exp_avg_sq[base + e];
+        w = adam_update(w, gr, m, v, lr_neg_step, beta1_w, beta2, beta2_w, eps, weight_decay, inv_bc2_sqrt);
+        exp_avg[base + e] = m;
+        exp_avg_sq[base + e] = v;
+        p[e] = w;
+      }
+      h += param_checksum_term(base + e, __float_as_uint(w));
+    }
+    base += n;
+  }
+  if (!skip) stamp_checksum(h, hdr);
+}
+
+static int repack_if_dirty(float* const* params, int precision, int new_activation, void* packed, cudaStream_t st) {
+  if (packed == nullptr) return SNB_OK;
+  const float* cp[SNB_N_PARAM_TENSORS];
+  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) cp[i] = params[i];
+  if (precision == SNB_PREC_FP32) return launch_pack_fp32(cp, new_activation ? 1 : 0, packed, 1, st);
+  return launch_pack_tc(cp, precision, new_activation ? 1 : 0, packed, 1, st);
+}
+
+static AmpCtl amp_ctl(const SnbAmpStep& amp) { return AmpCtl{amp.scale, amp.found_inf, amp.count_in, amp.count_out}; }
+
+int adam_step_pack_amp(float* const* params, float* const* grads, float* exp_avg, float* exp_avg_sq,
+                       const SnbAdamArgs& o, const SnbAmpStep& amp, int precision, int new_activation, void* packed,
+                       cudaStream_t st) {
+  AdamPtrs a;
+  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) { a.p[i] = params[i]; a.g[i] = grads[i]; }
+  AdamWindow win;
+  win.base = amp.base[0];
+  for (int j = 0; j < kOptimWindow; ++j)
+    adam_bias_scalars(o.lr, o.beta1, o.beta2, win.base + j, &win.lr_neg_step[j], &win.inv_bc2_sqrt[j]);
+  const float beta1_w = (float)(1.0 - o.beta1), beta2_w = (float)(1.0 - o.beta2);
+  adam_step_amp_kernel<<<sm_count() * 2, 256, 0, st>>>(a, exp_avg, exp_avg_sq, beta1_w, (float)o.beta2, beta2_w,
+                                                      (float)o.eps, (float)o.weight_decay, win, amp_ctl(amp),
+                                                      reinterpret_cast<PackedHeader*>(packed));
+  if (int rc = check_launch("adam_step_amp_kernel")) return rc;
+  return repack_if_dirty(params, precision, new_activation, packed, st);
+}
+
+// The window of one tensor: -step_size * lr and the flags at counts base .. base + kOptimWindow - 1.  Tensors at the
+// same base (all of them, unless some lacked a gradient on some steps) share the host arithmetic.
+static void rule_window(const SnbOptimArgs& o, int base, int* cached_base, float* step_lr, unsigned char* flags,
+                        const float* cached_lr, const unsigned char* cached_flags) {
+  if (*cached_base == base && cached_lr != nullptr) {
+    for (int j = 0; j < kOptimWindow; ++j) { step_lr[j] = cached_lr[j]; flags[j] = cached_flags[j]; }
+    return;
+  }
+  for (int j = 0; j < kOptimWindow; ++j) {
+    unsigned f;
+    rule_tensor_scalars(o, base + j, &step_lr[j], &f);
+    flags[j] = (unsigned char)f;
+  }
+  *cached_base = base;
+}
+
+// Whether tensor t's count advances on a taken step: it has a gradient, and the rule keeps a count (SGD only with
+// momentum, where the count says whether the momentum buffer exists yet).
+static bool rule_advances(const SnbOptimArgs& o, const void* grad) {
+  return grad != nullptr && (o.rule != SNB_OPTIM_SGD || o.momentum != 0.);
+}
+
+struct RuleWindow {
+  RuleConsts c;
+  unsigned adv;                                            // bit t: tensor t advances its count on a taken step
+  int base[SNB_N_PARAM_TENSORS];
+  float step_lr[SNB_N_PARAM_TENSORS][kOptimWindow];
+  unsigned char flags[SNB_N_PARAM_TENSORS][kOptimWindow];
+};
+
+template <int RULE>
+__global__ void __launch_bounds__(256) optim_step_amp_kernel(AdamPtrs a, float* __restrict__ exp_avg,
+                                                             float* __restrict__ exp_avg_sq,
+                                                             float* __restrict__ slow_buffer, RuleWindow s, AmpCtl amp,
+                                                             PackedHeader* hdr) {
+  const bool skip = amp_skip(amp.found_inf);
+  const float inv = amp_inv_scale(amp.scale);
+  if (blockIdx.x == 0) {
+    if (threadIdx.x < SNB_N_PARAM_TENSORS)
+      amp.count_out[threadIdx.x] = amp.count_in[threadIdx.x] + ((!skip && (s.adv >> threadIdx.x) & 1u) ? 1 : 0);
+    if (threadIdx.x == 0 && skip && hdr != nullptr) hdr->dirty = 0;
+  }
+  unsigned long long h = 0;
+  unsigned long long base = 0;
+  for (int t = 0; t < SNB_N_PARAM_TENSORS; ++t) {
+    const int n = param_numel(t);
+    float* p = a.p[t];
+    float* g = const_cast<float*>(a.g[t]);
+    unsigned f = 0;
+    float step_lr = 0.f;
+    if (!skip && ((s.adv >> t) & 1u)) {
+      const int j = amp.count_in[t] + 1 - s.base[t];
+      f = s.flags[t][j];
+      step_lr = s.step_lr[t][j];
+    }
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
+      const float gr = g != nullptr ? amp_unscale(g, e, inv) : 0.f;
+      if (skip) continue;
+      float w = p[e];
+      if (g != nullptr) {
+        w = rule_update<RULE>(w, gr, base + e, exp_avg, exp_avg_sq, slow_buffer, s.c, f, step_lr);
+        p[e] = w;
+      }
+      h += param_checksum_term(base + e, __float_as_uint(w));
+    }
+    base += n;
+  }
+  if (!skip) stamp_checksum(h, hdr);
+}
+
+int optim_step_pack_amp(float* const* params, float* const* grads, float* exp_avg, float* exp_avg_sq,
+                        float* slow_buffer, const SnbOptimArgs& o, const SnbAmpStep& amp, int precision,
+                        int new_activation, void* packed, cudaStream_t st) {
+  AdamPtrs a;
+  for (int i = 0; i < SNB_N_PARAM_TENSORS; ++i) { a.p[i] = params[i]; a.g[i] = grads[i]; }
+  RuleWindow s = {};
+  s.c = rule_consts(o);
+  int cached = -1, prev = -1;
+  for (int t = 0; t < SNB_N_PARAM_TENSORS; ++t) {
+    s.base[t] = amp.base[t];
+    if (!rule_advances(o, grads[t])) continue;
+    s.adv |= 1u << t;
+    rule_window(o, amp.base[t], &cached, s.step_lr[t], s.flags[t], prev < 0 ? nullptr : s.step_lr[prev],
+                prev < 0 ? nullptr : s.flags[prev]);
+    prev = t;
+  }
+  PackedHeader* hdr = reinterpret_cast<PackedHeader*>(packed);
+  const AmpCtl ctl = amp_ctl(amp);
+  const int grid = sm_count() * 2;
+  if (o.rule == SNB_OPTIM_SGD)
+    optim_step_amp_kernel<SNB_OPTIM_SGD><<<grid, 256, 0, st>>>(a, exp_avg, exp_avg_sq, slow_buffer, s, ctl, hdr);
+  else if (o.rule == SNB_OPTIM_RADAM)
+    optim_step_amp_kernel<SNB_OPTIM_RADAM><<<grid, 256, 0, st>>>(a, exp_avg, exp_avg_sq, slow_buffer, s, ctl, hdr);
+  else
+    optim_step_amp_kernel<SNB_OPTIM_RANGER><<<grid, 256, 0, st>>>(a, exp_avg, exp_avg_sq, slow_buffer, s, ctl, hdr);
+  if (int rc = check_launch("optim_step_amp_kernel")) return rc;
+  return repack_if_dirty(params, precision, new_activation, packed, st);
+}
+
+// The table of snb_optim_step_tensors_amp: as TensorTable, with each entry's scalars over its window and the index of
+// its count (entries are only the tensors with a gradient; counts cover all n_all tensors).
+struct TensorEntryAmp {
+  float* p;
+  float* g;
+  long long n;
+  unsigned long long off;
+  int slot;                            // index into the count arrays
+  int base;
+  float step_lr[kOptimWindow];         // Adam: -lr / (1 - beta1^t);  RAdam / Ranger: -step_size * lr
+  float inv_bc2_sqrt[kOptimWindow];    // Adam: 1 / sqrt(1 - beta2^t)
+  unsigned char flags[kOptimWindow];   // SGD / RAdam / Ranger: kFirst | kAdaptive | kSync
+};
+
+struct TensorTableAmp {
+  TensorEntryAmp t[SNB_OPTIM_MAX_TENSORS];
+  int n;
+  int n_all;
+  unsigned adv;                        // bit i: tensor i advances its count on a taken step
+};
+
+template <int RULE>
+__global__ void __launch_bounds__(256) optim_tensors_amp_kernel(TensorTableAmp tab, float* __restrict__ exp_avg,
+                                                                float* __restrict__ exp_avg_sq,
+                                                                float* __restrict__ slow_buffer, RuleConsts c,
+                                                                AmpCtl amp) {
+  const bool skip = amp_skip(amp.found_inf);
+  const float inv = amp_inv_scale(amp.scale);
+  if (blockIdx.x == 0 && threadIdx.x < tab.n_all)
+    amp.count_out[threadIdx.x] = amp.count_in[threadIdx.x] + ((!skip && (tab.adv >> threadIdx.x) & 1u) ? 1 : 0);
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (int t = 0; t < tab.n; ++t) {
+    float* p = tab.t[t].p;
+    float* g = tab.t[t].g;
+    const long long n = tab.t[t].n;
+    const unsigned long long off = tab.t[t].off;
+    float step_lr = 0.f, inv_bc2_sqrt = 0.f;
+    unsigned f = 0;
+    if (!skip && ((tab.adv >> tab.t[t].slot) & 1u)) {
+      const int j = amp.count_in[tab.t[t].slot] + 1 - tab.t[t].base;
+      step_lr = tab.t[t].step_lr[j];
+      inv_bc2_sqrt = tab.t[t].inv_bc2_sqrt[j];
+      f = tab.t[t].flags[j];
+    }
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += stride) {
+      const float gr = amp_unscale(g, e, inv);
+      if (skip) continue;
+      const unsigned long long i = off + e;
+      if (RULE == SNB_OPTIM_ADAM) {
+        float m = exp_avg[i], v = exp_avg_sq[i];
+        p[e] = adam_update(p[e], gr, m, v, step_lr, c.beta1_w, c.beta2, c.beta2_w, c.eps, c.decay, inv_bc2_sqrt);
+        exp_avg[i] = m;
+        exp_avg_sq[i] = v;
+      } else {
+        p[e] = rule_update<RULE>(p[e], gr, i, exp_avg, exp_avg_sq, slow_buffer, c, f, step_lr);
+      }
+    }
+  }
+}
+
+int optim_step_tensors_amp(int n, float* const* params, float* const* grads, const int64_t* numel, float* exp_avg,
+                           float* exp_avg_sq, float* slow_buffer, const SnbOptimArgs& o, const SnbAmpStep& amp,
+                           cudaStream_t st) {
+  TensorTableAmp tab = {};
+  tab.n_all = n;
+  unsigned long long off = 0;
+  int cached = -1;
+  const TensorEntryAmp* prev = nullptr;
+  for (int t = 0; t < n; off += (unsigned long long)numel[t], ++t) {
+    if (grads[t] == nullptr) continue;
+    TensorEntryAmp& te = tab.t[tab.n++];
+    te.p = params[t];
+    te.g = grads[t];
+    te.n = numel[t];
+    te.off = off;
+    te.slot = t;
+    te.base = amp.base[t];
+    if (!rule_advances(o, grads[t])) continue;
+    tab.adv |= 1u << t;
+    if (o.rule == SNB_OPTIM_ADAM) {
+      for (int j = 0; j < kOptimWindow; ++j)
+        adam_bias_scalars(o.lr, o.beta1, o.beta2, te.base + j, &te.step_lr[j], &te.inv_bc2_sqrt[j]);
+    } else {
+      rule_window(o, te.base, &cached, te.step_lr, te.flags, prev ? prev->step_lr : nullptr,
+                  prev ? prev->flags : nullptr);
+      prev = &te;
+    }
+  }
+  const RuleConsts c = rule_consts(o);
+  const AmpCtl ctl = amp_ctl(amp);
+  const int grid = tab.n == 0 ? 1 : sm_count() * 4;   // with no gradient at all, one block still copies the counts
+  if (o.rule == SNB_OPTIM_ADAM)
+    optim_tensors_amp_kernel<SNB_OPTIM_ADAM><<<grid, 256, 0, st>>>(tab, exp_avg, exp_avg_sq, slow_buffer, c, ctl);
+  else if (o.rule == SNB_OPTIM_SGD)
+    optim_tensors_amp_kernel<SNB_OPTIM_SGD><<<grid, 256, 0, st>>>(tab, exp_avg, exp_avg_sq, slow_buffer, c, ctl);
+  else if (o.rule == SNB_OPTIM_RADAM)
+    optim_tensors_amp_kernel<SNB_OPTIM_RADAM><<<grid, 256, 0, st>>>(tab, exp_avg, exp_avg_sq, slow_buffer, c, ctl);
+  else
+    optim_tensors_amp_kernel<SNB_OPTIM_RANGER><<<grid, 256, 0, st>>>(tab, exp_avg, exp_avg_sq, slow_buffer, c, ctl);
+  return check_launch("optim_tensors_amp_kernel");
+}
+
 }  // namespace snb

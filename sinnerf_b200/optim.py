@@ -18,9 +18,18 @@ launch of snb_optim_step_tensors, with no re-pack (the discriminator derives its
 call).  There Adam too keeps a step count per parameter, and every rule creates a parameter's state on its first step,
 as torch.optim.Adam / SGD and the reference's RAdam / Ranger do over `D.parameters()`; so `opt_d`'s state dict moves
 both ways between them and the fused optimisers.
+
+Under AMP all four set `_step_supports_amp_scaling`, so `scaler.step(opt)` hands them GradScaler's scale and found_inf
+as device tensors and does not wait for found_inf on the host: the step kernel unscales each gradient (writing it back
+to `.grad`, as GradScaler.unscale_ would) and skips the update itself when found_inf is set.  The update counts the
+step-dependent scalars need then live on the device (`_Counts`); `state`, `state_dict()` and `load_state_dict()` read
+them back when they are behind, so they return what the plain path returns after the same taken and skipped steps.
+`amp_scaling=False` keeps GradScaler's own unscale pass and its host check of found_inf (Lightning refuses gradient
+clipping for optimisers that unscale internally).
 """
 from __future__ import annotations
 
+import collections
 import ctypes as C
 from typing import Iterable, Optional
 
@@ -62,39 +71,169 @@ def _check_tensors(ps, who: str) -> None:
             raise ValueError(f"{who}: a module's parameters must be on one device (got {p.device} and {ps[0].device})")
 
 
+class _Counts:
+    """The update counts of one module's tensors (FusedAdam over a NeRF: one count for the module) as GradScaler-native
+    steps leave them: on the device, where the kernel advances them only on a taken step, with the host's view a
+    step or more behind.
+
+    `host` holds the counts as last read back, `lag` the increments issued since, any of which may have been skipped.
+    Each step's kernel reads the counts from one row of `dev` and writes them to the other.  Right after the launch the
+    new row is copied to pinned memory without blocking; a later step picks up the newest copy whose event has
+    completed.  A step needs lag < OPTIM_WINDOW on every count it advances, because the kernel's table of scalars
+    covers the counts host + 1 .. host + OPTIM_WINDOW.  Only when the GPU runs that many steps behind does it wait for
+    one copy.  Plain steps and loaded state change `host` directly; the device row is refreshed from it before the
+    next GradScaler-native step."""
+
+    def __init__(self, n: int):
+        self.host = [0] * n
+        self.lag = [0] * n
+        self.issued = [0] * n          # increments issued in all, to match a read-back with the steps after it
+        self.dev = None                # (2, n) int32 on the module's device
+        self.row = 0                   # the row holding the current counts
+        self.dev_current = False       # whether the device rows follow `host` (False after a host-side change)
+        self.reads = collections.deque()   # in-flight read-backs: (event, pinned row, issued at the copy)
+        self.ring = self.events = None
+        self.seq = 0
+
+    def exact(self) -> bool:
+        return not any(self.lag)
+
+    def poll(self) -> None:
+        """Take the newest completed read-back, without waiting."""
+        done = None
+        while self.reads and self.reads[0][0].query():
+            done = self.reads.popleft()
+        if done is not None:
+            self.host = done[1].tolist()
+            self.lag = [a - b for a, b in zip(self.issued, done[2])]
+
+    def settle(self) -> None:
+        """Make `host` exact: the newest completed read-back, or one blocking copy when that is behind."""
+        self.poll()
+        if not self.exact():
+            self.host = self.dev[self.row].tolist()
+            self.lag = [0] * len(self.host)
+        self.reads.clear()
+
+    def load(self, counts) -> None:
+        """Counts set on the host (a plain step, a loaded state dict); `host` must be exact."""
+        assert self.exact()
+        self.host = list(counts)
+        self.dev_current = False
+        self.reads.clear()
+
+    def prepare(self, advances, dev) -> list:
+        """Before a GradScaler-native step: the device rows current and the window in reach of every count the step
+        advances.  Returns the window bases."""
+        self.poll()
+        if any(a and lag >= _lib.OPTIM_WINDOW for a, lag in zip(advances, self.lag)):
+            self.settle()
+        if not self.dev_current:
+            if self.dev is None:
+                n = len(self.host)
+                self.dev = torch.zeros(2, n, dtype=torch.int32, device=dev)
+                self.ring = torch.empty(_lib.OPTIM_WINDOW, n, dtype=torch.int32, pin_memory=True)
+                self.events = [torch.cuda.Event() for _ in range(_lib.OPTIM_WINDOW)]
+            self.dev[self.row].copy_(torch.tensor(self.host, dtype=torch.int32).pin_memory(), non_blocking=True)
+            self.dev_current = True
+        return [c + 1 for c in self.host]
+
+    def pointers(self):
+        return _lib.ptr(self.dev[self.row]), _lib.ptr(self.dev[self.row ^ 1])
+
+    def advance(self, advances) -> None:
+        """After the launch: the kernel's output row is current; start reading it back."""
+        self.row ^= 1
+        for t, a in enumerate(advances):
+            if a:
+                self.issued[t] += 1
+                self.lag[t] += 1
+        if len(self.reads) < _lib.OPTIM_WINDOW:
+            k = self.seq % _lib.OPTIM_WINDOW
+            self.seq += 1
+            self.ring[k].copy_(self.dev[self.row], non_blocking=True)
+            self.events[k].record()
+            self.reads.append((self.events[k], self.ring[k], list(self.issued)))
+
+
+def _amp_tensor(t, dev):
+    """GradScaler's grad_scale / found_inf as a float32 tensor on dev; None where it is absent.  found_inf is the
+    integer 0 when no gradient was checked (nothing to skip for)."""
+    if not torch.is_tensor(t):
+        return None
+    return t.to(device=dev, dtype=torch.float32, non_blocking=True)
+
+
 class _FusedPerTensor(torch.optim.Optimizer):
     """Shared body of FusedSGD / FusedRAdam / FusedRanger (C ABI snb_optim_step): one kernel per model and step, then
     the re-pack of the weight image on the same stream.  For Discriminator modules (and FusedAdam over them): one
     snb_optim_step_tensors launch per module and step, nothing to re-pack.
 
     These rules keep a step count per parameter and skip parameters without a gradient, so the count is tracked per
-    tensor (`_count`) and passed to the kernel per tensor.  State mirrors the reference's exactly: a parameter has a
+    tensor (`_counts`, one `_Counts` per module) and passed to the kernel per tensor.  State mirrors the reference's exactly: a parameter has a
     `state` entry only once it has been stepped, holding views of the flat buffers the kernel updates."""
     _rule: int
     _buffers: tuple          # state keys of the flat buffers, in snb_optim_step's argument order
     _has_step: bool = True   # the state carries the reference's per-parameter `step`
+    _step_supports_amp_scaling = True   # GradScaler passes grad_scale / found_inf instead of unscaling and syncing
 
-    def __init__(self, models: Iterable, defaults: dict, precision: Optional[str]):
+    def __init__(self, models: Iterable, defaults: dict, precision: Optional[str], amp_scaling: bool = True):
         self.models, self._disc = _check_modules(models, type(self).__name__)
         super().__init__([p for m in self.models for p in _params(m)], defaults)
         self._precision = precision
+        if not amp_scaling:
+            self._step_supports_amp_scaling = False
         self._flat = []          # per model: the flat state buffers, in _buffers order
         self._views = {}         # parameter -> {state key: view of its slice of the flat buffer}
-        self._count = {}         # parameter -> updates applied so far (the reference's state['step'])
+        self._slot = {}          # parameter -> (model index, tensor index): where its update count is kept
+        self._counts = [_Counts(self._n_counts(m)) for m in self.models]   # the reference's state['step'] per tensor
+        self._stale = False      # GradScaler-native steps ran since `state` was last published
+
+    def _n_counts(self, m) -> int:
+        return len(_params(m))
+
+    @property
+    def state(self):
+        """torch.optim.Optimizer's `state`, brought up to date with the device's update counts first."""
+        self._sync()
+        return self.__dict__["state"]
+
+    @state.setter
+    def state(self, value):
+        self.__dict__["state"] = value
+
+    def _sync(self) -> None:
+        if self.__dict__.get("_stale"):
+            self._stale = False
+            for c in self._counts:
+                c.settle()
+            self._publish()
+
+    def _count(self, p) -> int:
+        i, t = self._slot[p]
+        return self._counts[i].host[t]
+
+    def _amp_inputs(self, dev):
+        """(grad_scale, found_inf) as GradScaler's step() attached them, on dev, or None outside GradScaler-native
+        stepping (a plain opt.step(), a disabled scaler, amp_scaling=False).  grad_scale is None after
+        scaler.unscale_(opt): the gradients are unscaled already."""
+        if not self._step_supports_amp_scaling or not hasattr(self, "found_inf"):
+            return None
+        return _amp_tensor(getattr(self, "grad_scale", None), dev), _amp_tensor(self.found_inf, dev)
 
     def _ensure_state(self):
         if self._flat:
             return
-        for m in self.models:
+        for i, m in enumerate(self.models):
             ps = _params(m)
             _lib.require_device(ps[0], type(self).__name__)
             total = sum(p.numel() for p in ps)
             bufs = [torch.zeros(total, device=ps[0].device, dtype=torch.float32) for _ in self._buffers]
             off = 0
-            for p in ps:
+            for t, p in enumerate(ps):
                 n = p.numel()
                 self._views[p] = {k: b[off:off + n].view_as(p) for k, b in zip(self._buffers, bufs)}
-                self._count[p] = 0
+                self._slot[p] = (i, t)
                 off += n
             assert self._disc or off == _lib.PARAM_FLOATS
             self._flat.append(bufs)
@@ -104,26 +243,35 @@ class _FusedPerTensor(torch.optim.Optimizer):
         return n
 
     def _publish(self):
-        self.state.clear()
-        for p, n in self._count.items():
+        state = self.__dict__["state"]
+        state.clear()
+        for p in self._views:
+            n = self._count(p)
             if n > 0:
-                self.state[p] = dict(self._views[p], **({"step": self._step_value(n)} if self._has_step else {}))
+                state[p] = dict(self._views[p], **({"step": self._step_value(n)} if self._has_step else {}))
 
     def load_state_dict(self, state_dict):
         """Values are copied INTO the flat buffers (the kernel addresses them by offset); a parameter without state
         starts afresh, as in the reference."""
         self._ensure_state()
+        self._sync()
+        for c in self._counts:
+            c.settle()
         super().load_state_dict(state_dict)
+        counts = [list(c.host) for c in self._counts]
         for p, views in self._views.items():
             st = self.state.get(p, {})
+            i, t = self._slot[p]
             if all(st.get(k) is not None for k in self._buffers):
                 for k, v in views.items():
                     v.copy_(st[k])
-                self._count[p] = int(st["step"]) if self._has_step else 1
+                counts[i][t] = int(st["step"]) if self._has_step else 1
             else:
                 for v in views.values():
                     v.zero_()
-                self._count[p] = 0
+                counts[i][t] = 0
+        for c, n in zip(self._counts, counts):
+            c.load(n)
         self._publish()
 
     def _args(self, group) -> "_lib.SnbOptimArgs":
@@ -144,31 +292,64 @@ class _FusedPerTensor(torch.optim.Optimizer):
         group = self.param_groups[0]
         args = self._args(group)
         adv = self._advances(group)
-        for m, bufs in zip(self.models, self._flat):
+        amp_step = False
+        for m, bufs, counts in zip(self.models, self._flat, self._counts):
             ps = _params(m)
             dev = ps[0].device
             _check_tensors(ps, type(self).__name__)
-            for p in ps:
-                if p.grad is not None and adv:
-                    self._count[p] += 1
+            advances = [p.grad is not None and adv for p in ps]
             parr = (C.c_void_p * len(ps))(*[p.data_ptr() for p in ps])
             garr = (C.c_void_p * len(ps))(*[(p.grad.data_ptr() if p.grad is not None else None) for p in ps])
             st = [_lib.ptr(b) for b in bufs] + [None] * (3 - len(bufs))
+            amp = self._amp_inputs(dev)
+            if amp is not None:
+                amp_step = True
+                with torch.cuda.device(dev):
+                    ctl = self._amp_ctl(counts, advances, amp, dev)
+                    if self._disc:
+                        _lib.check(lib.snb_optim_step_tensors_amp(len(ps), parr, garr,
+                                                                  (C.c_int64 * len(ps))(*[p.numel() for p in ps]), *st,
+                                                                  C.byref(args), C.byref(ctl), _lib.stream_ptr(dev)),
+                                   "snb_optim_step_tensors_amp")
+                    else:
+                        prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
+                        image = m.packed_image_buffer(prec)
+                        _lib.check(lib.snb_optim_step_amp(parr, garr, *st, C.byref(args), C.byref(ctl), prec,
+                                                          int(m.use_new_activation), _lib.ptr(image),
+                                                          _lib.stream_ptr(dev)), "snb_optim_step_amp")
+                    counts.advance(advances)
+                continue
+            counts.settle()
+            counts.load([c + 1 if a else c for c, a in zip(counts.host, advances)])
             with torch.cuda.device(dev):
                 if self._disc:
                     _lib.check(lib.snb_optim_step_tensors(len(ps), parr, garr,
                                                           (C.c_int64 * len(ps))(*[p.numel() for p in ps]),
-                                                          (C.c_int * len(ps))(*[self._count[p] for p in ps]), *st,
+                                                          (C.c_int * len(ps))(*counts.host), *st,
                                                           C.byref(args), _lib.stream_ptr(dev)), "snb_optim_step_tensors")
                     continue
                 prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
-                for i, p in enumerate(ps):
-                    args.step[i] = self._count[p]
+                for i, c in enumerate(counts.host):
+                    args.step[i] = c
                 image = m.packed_image_buffer(prec)
                 _lib.check(lib.snb_optim_step(parr, garr, *st, C.byref(args), prec, int(m.use_new_activation),
                                               _lib.ptr(image), _lib.stream_ptr(dev)), "snb_optim_step")
-        self._publish()
+        if amp_step:
+            self._stale = True
+        else:
+            self._publish()
         return loss
+
+    @staticmethod
+    def _amp_ctl(counts: _Counts, advances, amp, dev) -> "_lib.SnbAmpStep":
+        """The SnbAmpStep of one module's GradScaler-native step: the device scale and found_inf, the count rows,
+        and the window bases."""
+        base = counts.prepare(advances, dev)
+        count_in, count_out = counts.pointers()
+        ctl = _lib.SnbAmpStep(scale=_lib.ptr(amp[0]), found_inf=_lib.ptr(amp[1]), count_in=count_in,
+                              count_out=count_out)
+        ctl.base[:len(base)] = base
+        return ctl
 
 
 class FusedAdam(_FusedPerTensor):
@@ -180,12 +361,25 @@ class FusedAdam(_FusedPerTensor):
     _buffers = ("exp_avg", "exp_avg_sq")
 
     def __init__(self, models: Iterable, lr: float = 5e-4, betas=(0.9, 0.999), eps: float = 1e-8,
-                 weight_decay: float = 0.0, precision: Optional[str] = None):
-        super().__init__(models, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), precision)
-        self._steps = 0          # NeRF models: updates applied so far
+                 weight_decay: float = 0.0, precision: Optional[str] = None, amp_scaling: bool = True):
+        super().__init__(models, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), precision, amp_scaling)
+
+    def _n_counts(self, m):
+        return len(_params(m)) if self._disc else 1
+
+    @property
+    def _steps(self) -> int:
+        """NeRF models: updates applied so far (one count per model; all models step together)."""
+        return self._counts[0].host[0]
 
     def _step_value(self, n):
         return torch.tensor(float(n))
+
+    def _publish(self):
+        if self._disc:
+            return super()._publish()
+        for st in self.__dict__["state"].values():
+            st["step"] = torch.tensor(float(self._steps))
 
     def _args(self, group):
         return _lib.SnbOptimArgs(rule=self._rule, lr=float(group["lr"]), weight_decay=float(group["weight_decay"]),
@@ -206,8 +400,9 @@ class FusedAdam(_FusedPerTensor):
             off = 0
             for p in ps:
                 n = p.numel()
-                self.state[p] = {"step": torch.tensor(float(self._steps)), "exp_avg": ea[off:off + n].view_as(p),
-                                 "exp_avg_sq": es[off:off + n].view_as(p)}
+                self.__dict__["state"][p] = {"step": torch.tensor(float(self._steps)),
+                                             "exp_avg": ea[off:off + n].view_as(p),
+                                             "exp_avg_sq": es[off:off + n].view_as(p)}
                 off += n
             assert off == _lib.PARAM_FLOATS
             self._flat.append((ea, es))
@@ -218,6 +413,8 @@ class FusedAdam(_FusedPerTensor):
             return super().load_state_dict(state_dict)
         self._ensure_state()
         views = {id(p): dict(st) for p, st in self.state.items()}
+        for c in self._counts:
+            c.settle()
         torch.optim.Optimizer.load_state_dict(self, state_dict)
         step = 0
         for p, st in self.state.items():
@@ -226,7 +423,8 @@ class FusedAdam(_FusedPerTensor):
                 keep[k].copy_(st[k])
                 st[k] = keep[k]
             step = max(step, int(float(st.get("step", 0))))
-        self._steps = step
+        for c in self._counts:
+            c.load([step])
 
     @torch.no_grad()
     def step(self, closure=None):
@@ -239,10 +437,10 @@ class FusedAdam(_FusedPerTensor):
         self._ensure_state()
         lib = _lib.load()
         g = self.param_groups[0]
-        self._steps += 1
+        amp_step = False
         args = _lib.SnbAdamArgs(float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]),
-                                float(g["weight_decay"]), self._steps)
-        for m, (ea, es) in zip(self.models, self._flat):
+                                float(g["weight_decay"]), 0)
+        for m, (ea, es), counts in zip(self.models, self._flat, self._counts):
             prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
             ps = m._param_list()
             dev = ps[0].device
@@ -250,12 +448,26 @@ class FusedAdam(_FusedPerTensor):
             image = m.packed_image_buffer(prec)
             parr = (C.c_void_p * 24)(*[p.data_ptr() for p in ps])
             garr = (C.c_void_p * 24)(*[(p.grad.data_ptr() if p.grad is not None else None) for p in ps])
+            amp = self._amp_inputs(dev)
             with torch.cuda.device(dev):
+                if amp is not None:
+                    amp_step = True
+                    ctl = self._amp_ctl(counts, [True], amp, dev)
+                    _lib.check(lib.snb_adam_step_amp(parr, garr, _lib.ptr(ea), _lib.ptr(es), C.byref(args),
+                                                     C.byref(ctl), prec, int(m.use_new_activation), _lib.ptr(image),
+                                                     _lib.stream_ptr(dev)), "snb_adam_step_amp")
+                    counts.advance([True])
+                    continue
+                counts.settle()
+                counts.load([counts.host[0] + 1])
+                args.step = counts.host[0]
                 _lib.check(lib.snb_adam_step(parr, garr, _lib.ptr(ea), _lib.ptr(es), C.byref(args), prec,
                                              int(m.use_new_activation), _lib.ptr(image), _lib.stream_ptr(dev)),
                            "snb_adam_step")
-        for st in self.state.values():
-            st["step"] = torch.tensor(float(self._steps))
+        if amp_step:
+            self._stale = True
+        else:
+            self._publish()
         return loss
 
 
@@ -268,9 +480,10 @@ class FusedSGD(_FusedPerTensor):
     _has_step = False
 
     def __init__(self, models: Iterable, lr: float, momentum: float = 0.0, weight_decay: float = 0.0,
-                 precision: Optional[str] = None):
+                 precision: Optional[str] = None,
+                 amp_scaling: bool = True):
         super().__init__(models, dict(lr=lr, momentum=momentum, dampening=0.0, weight_decay=weight_decay,
-                                      nesterov=False), precision)
+                                      nesterov=False), precision, amp_scaling)
 
     def _advances(self, group):
         return group["momentum"] != 0
@@ -290,9 +503,10 @@ class FusedRAdam(_FusedPerTensor):
     _buffers = ("exp_avg", "exp_avg_sq")
 
     def __init__(self, models: Iterable, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
-                 weight_decay: float = 0.0, precision: Optional[str] = None):
+                 weight_decay: float = 0.0, precision: Optional[str] = None,
+                 amp_scaling: bool = True):
         super().__init__(models, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
-                                      buffer=[[None, None, None] for _ in range(10)]), precision)
+                                      buffer=[[None, None, None] for _ in range(10)]), precision, amp_scaling)
 
     def _args(self, group):
         return _lib.SnbOptimArgs(rule=self._rule, lr=float(group["lr"]), weight_decay=float(group["weight_decay"]),
@@ -309,9 +523,10 @@ class FusedRanger(_FusedPerTensor):
 
     def __init__(self, models: Iterable, lr: float = 1e-3, alpha: float = 0.5, k: int = 6,
                  N_sma_threshhold: float = 5, betas=(0.95, 0.999), eps: float = 1e-5, weight_decay: float = 0.0,
-                 precision: Optional[str] = None):
+                 precision: Optional[str] = None,
+                 amp_scaling: bool = True):
         super().__init__(models, dict(lr=lr, alpha=alpha, k=k, step_counter=0, betas=betas,
-                                      N_sma_threshhold=N_sma_threshhold, eps=eps, weight_decay=weight_decay), precision)
+                                      N_sma_threshhold=N_sma_threshhold, eps=eps, weight_decay=weight_decay), precision, amp_scaling)
 
     def _args(self, group):
         return _lib.SnbOptimArgs(rule=self._rule, lr=float(group["lr"]), weight_decay=float(group["weight_decay"]),
