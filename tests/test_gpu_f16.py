@@ -14,6 +14,7 @@ import torch
 from oracle import render_oracle as orc
 from tests import f16_oracle
 from tests._common import rel_l2, room_params
+from tests.test_gpu_field_schedule import ENTRIES
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -121,9 +122,9 @@ def schedule_checks(monkeypatch):
     return fs
 
 
-@pytest.mark.parametrize("sigma_only", [False, True])
-def test_field_rows_independent_of_tile_offset(schedule_checks, sigma_only):
-    schedule_checks.test_field_rows_independent_of_tile_offset("f16", sigma_only)
+@pytest.mark.parametrize("sigma_only,storage", ENTRIES)
+def test_field_rows_independent_of_tile_offset(schedule_checks, sigma_only, storage):
+    schedule_checks.test_field_rows_independent_of_tile_offset("f16", sigma_only, storage)
 
 
 @pytest.mark.parametrize("sigma_only", [False, True])
@@ -150,29 +151,13 @@ F16_BOUNDS = (5.0e-6, 9.0e-6, 2.0e-6, 7.0e-6, 3.0e-6, 5.0e-7)
 assert F16_BOUNDS[0] * 50 <= 2.0 ** -11
 
 
-@pytest.fixture
-def layerwise_f16(monkeypatch):
-    from tests import test_gpu_layerwise as tl
-    operand = tl.operand
-
-    def operand_f16(x, mode, nonneg=False):
-        if mode != "f16":
-            return operand(x, mode, nonneg)
-        x = x.float()
-        x = x.clamp(max=65504.0) if nonneg else x.clamp(-65504.0, 65504.0)
-        return x.half().float(), None
-
-    monkeypatch.setattr(tl, "operand", operand_f16)
-    monkeypatch.setitem(tl.FWD_BOUNDS, "f16", F16_BOUNDS)
-    return tl
-
-
 @pytest.mark.parametrize("tag", ["default", "room"])
-def test_training_forward_layerwise(layerwise_f16, tag):
+def test_training_forward_layerwise(tag):
     """Every saved tensor of snb_field_forward_train in f16 against float64 from the kernel's own saved inputs, their
     MMA operands rounded to nearest fp16: 4096 lego rays x 128 samples and a ragged DTU batch."""
-    layerwise_f16.check_forward_layers("f16", tag, "lego", 4096, 128, 21)
-    layerwise_f16.check_forward_layers("f16", tag, "dtu", 333, 97, 22)
+    from tests import test_gpu_layerwise as tl
+    tl.check_forward_layers("f16", tag, "lego", 4096, 128, 21, bounds=F16_BOUNDS)
+    tl.check_forward_layers("f16", tag, "dtu", 333, 97, 22, bounds=F16_BOUNDS)
 
 
 # --------------------------------------------------------------------------------------------------------------------
