@@ -13,8 +13,9 @@
 // False), operation for operation, every elementwise op rounded to fp32 like the separate ATen kernels:
 //   g   = grad + weight_decay * p                         (add, alpha)
 //   m   = m + (1 - beta1) * (g - m)                       (lerp, weight < 0.5)
-//   v   = v * beta2;  v = v + (1 - beta2) * g * g         (mul_, addcmul_)
-//   den = sqrt(v) / sqrt(1 - beta2^t) + eps               (ATen divides by a CPU scalar as * (1 / scalar))
+//   v   = v * beta2;  v = v + (1 - beta2) * (g * g)       (mul_, addcmul_: ATen rounds the product g * g first)
+//   den = sqrt(v) / sqrt(1 - beta2^t) + eps               (division by a python float: * (1 / scalar), the reciprocal
+//                                                          formed in double and rounded to fp32 once)
 //   p   = p + (-lr / (1 - beta1^t)) * (m / den)           (addcdiv_)
 // Roofline: HBM/L2, 16 B read + 12 B written per parameter (17 MB per model) -- a few microseconds.
 #include "common.cuh"
@@ -58,7 +59,7 @@ __device__ __forceinline__ float adam_update(float w, float gr, float& m, float&
   if (weight_decay != 0.f) gr = fmaf(weight_decay, w, gr);
   m = fmaf(beta1_w, gr - m, m);
   v = __fmul_rn(v, beta2);
-  v = fmaf(__fmul_rn(beta2_w, gr), gr, v);
+  v = fmaf(beta2_w, __fmul_rn(gr, gr), v);
   const float den = __fadd_rn(__fmul_rn(__fsqrt_rn(v), inv_bc2_sqrt), eps);
   return fmaf(lr_neg_step, __fdiv_rn(m, den), w);
 }
@@ -99,12 +100,13 @@ static int repack(float* const* params, int precision, int new_activation, void*
 }
 
 // Adam's step-dependent scalars exactly as torch forms them: python doubles, cast to float where the kernels consume
-// them.  -lr / (1 - beta1^t) and 1 / sqrt(1 - beta2^t).
+// them.  -lr / (1 - beta1^t), and 1 / (1 - beta2^t) ** 0.5 with the reciprocal taken in double: a float reciprocal of
+// the float cast rounds twice and differs from torch's by an ulp at most counts (at t = 1: 31.622778 vs 31.622776).
 static void adam_bias_scalars(double lr, double beta1, double beta2, int step, float* lr_neg_step, float* inv_bc2_sqrt) {
   const double bc1 = 1.0 - pow(beta1, (double)step);
   const double bc2 = 1.0 - pow(beta2, (double)step);
   *lr_neg_step = (float)(-(lr / bc1));
-  *inv_bc2_sqrt = 1.0f / (float)sqrt(bc2);
+  *inv_bc2_sqrt = (float)(1.0 / pow(bc2, 0.5));
 }
 
 int adam_step_pack(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
@@ -123,13 +125,14 @@ int adam_step_pack(float* const* params, const float* const* grads, float* exp_a
 
 // ---------------------------------------------------------------- SGD / RAdam / Ranger (snb_optim_step)
 // Each line is one ATen elementwise kernel of the reference's step, rounded to fp32 as that kernel rounds it
-// (ATen's CUDA add / addcmul / addcdiv contract `a + alpha * b` into one FMA; mul, sqrt, div round on their own):
+// (ATen's CUDA add / addcmul / addcdiv contract `a + alpha * b` into one FMA, with b = t1 * t2 or t1 / t2 rounded on
+// its own for addcmul / addcdiv; mul, sqrt, div round on their own):
 //   SGD (torch/optim/sgd.py _multi_tensor_sgd, dampening 0, no Nesterov):
 //     g = g + wd * p                 (_foreach_add, alpha)
 //     b = g (first step)  |  b = b * momentum;  b = b + g         (_foreach_mul_, _foreach_add_)
 //     p = p + (-lr) * b              (_foreach_add_, alpha)
 //   RAdam / Ranger (utils/optimizers.py:65-66,90-104 / :393-425):
-//     v = v * beta2;  v = v + (1 - beta2) * g * g                 (mul_, addcmul_)
+//     v = v * beta2;  v = v + (1 - beta2) * (g * g)               (mul_, addcmul_)
 //     m = m * beta1;  m = m + (1 - beta1) * g                     (mul_, add_)
 //     p = p + (-wd * lr) * p                                      (add_, when wd != 0)
 //     p = p + (-step_size * lr) * (m / (sqrt(v) + eps))  if N_sma passes the threshold,   (sqrt, add_, addcdiv_)
@@ -166,7 +169,7 @@ __device__ __forceinline__ float rule_update(float w, float gr, unsigned long lo
     return fmaf(s.lr_neg, gr, w);
   }
   float v = __fmul_rn(exp_avg_sq[i], s.beta2);
-  v = fmaf(__fmul_rn(s.beta2_w, gr), gr, v);
+  v = fmaf(s.beta2_w, __fmul_rn(gr, gr), v);
   float m = __fmul_rn(exp_avg[i], s.beta1);
   m = fmaf(s.beta1_w, gr, m);
   exp_avg[i] = m;
