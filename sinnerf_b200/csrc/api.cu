@@ -69,17 +69,8 @@ int field_backward16(const float* const*, float* const*, int, const float*, cons
                      const float*, cudaStream_t);
 int field_backward16_sigma(const float* const*, float* const*, const float*, const void*, long long, void*, const float*,
                            cudaStream_t);
-int adam_step_pack(float* const*, const float* const*, float*, float*, const SnbAdamArgs&, int, int, void*, cudaStream_t);
-int optim_step_pack(float* const*, const float* const*, float*, float*, float*, const SnbOptimArgs&, int, int, void*,
-                    cudaStream_t);
-int optim_step_tensors(int, float* const*, const float* const*, const int64_t*, const int*, float*, float*, float*,
-                       const SnbOptimArgs&, cudaStream_t);
-int adam_step_pack_amp(float* const*, float* const*, float*, float*, const SnbAdamArgs&, const SnbAmpStep&, int, int,
-                       void*, cudaStream_t);
-int optim_step_pack_amp(float* const*, float* const*, float*, float*, float*, const SnbOptimArgs&, const SnbAmpStep&,
-                        int, int, void*, cudaStream_t);
-int optim_step_tensors_amp(int, float* const*, float* const*, const int64_t*, float*, float*, float*,
-                           const SnbOptimArgs&, const SnbAmpStep&, cudaStream_t);
+int fused_step(int, const int64_t*, float* const*, const float* const*, bool, const int*, const SnbAmpStep*, float*,
+               float*, float*, const SnbOptimArgs&, int, int, void*, cudaStream_t);
 // tensor-core modes (field_tc.cu)
 size_t tc_packed_bytes(int precision);
 int field_forward_tc(const void*, int, const float*, const float*, int64_t, int, int, float*, cudaStream_t);
@@ -542,13 +533,26 @@ static int check_amp(const char* who, const SnbAmpStep* amp, int n) {
   return SNB_OK;
 }
 
+// snb_adam_step's hyper-parameters as the Adam rule of the shared step.
+static SnbOptimArgs adam_rule(const SnbAdamArgs& a) {
+  SnbOptimArgs o = {};
+  o.rule = SNB_OPTIM_ADAM;
+  o.lr = a.lr;
+  o.beta1 = a.beta1;
+  o.beta2 = a.beta2;
+  o.eps = a.eps;
+  o.weight_decay = a.weight_decay;
+  return o;
+}
+
 int snb_adam_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
                   const SnbAdamArgs* args, int precision, int new_activation, void* packed, void* stream) {
   if (int rc = check_adam_step("snb_adam_step", params, grads, exp_avg, exp_avg_sq, args, args ? &args->step : nullptr,
                                precision, packed))
     return rc;
-  return adam_step_pack(params, grads, exp_avg, exp_avg_sq, *args, precision, new_activation, packed,
-                        reinterpret_cast<cudaStream_t>(stream));
+  return fused_step(SNB_N_PARAM_TENSORS, nullptr, params, grads, true, &args->step, nullptr, exp_avg, exp_avg_sq,
+                    nullptr, adam_rule(*args), precision, new_activation, packed,
+                    reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_adam_step_amp(float* const* params, float* const* grads, float* exp_avg, float* exp_avg_sq,
@@ -557,8 +561,8 @@ int snb_adam_step_amp(float* const* params, float* const* grads, float* exp_avg,
   const char* who = "snb_adam_step_amp";
   if (int rc = check_amp(who, amp, 1)) return rc;
   if (int rc = check_adam_step(who, params, grads, exp_avg, exp_avg_sq, args, amp->base, precision, packed)) return rc;
-  return adam_step_pack_amp(params, grads, exp_avg, exp_avg_sq, *args, *amp, precision, new_activation, packed,
-                            reinterpret_cast<cudaStream_t>(stream));
+  return fused_step(SNB_N_PARAM_TENSORS, nullptr, params, grads, true, amp->base, amp, exp_avg, exp_avg_sq, nullptr,
+                    adam_rule(*args), precision, new_activation, packed, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_optim_step(float* const* params, const float* const* grads, float* exp_avg, float* exp_avg_sq,
@@ -567,8 +571,8 @@ int snb_optim_step(float* const* params, const float* const* grads, float* exp_a
   if (int rc = check_optim_step("snb_optim_step", params, reinterpret_cast<const void* const*>(grads), exp_avg,
                                 exp_avg_sq, slow_buffer, args, args ? args->step : nullptr, precision, packed))
     return rc;
-  return optim_step_pack(params, grads, exp_avg, exp_avg_sq, slow_buffer, *args, precision, new_activation, packed,
-                         reinterpret_cast<cudaStream_t>(stream));
+  return fused_step(SNB_N_PARAM_TENSORS, nullptr, params, grads, false, args->step, nullptr, exp_avg, exp_avg_sq,
+                    slow_buffer, *args, precision, new_activation, packed, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_optim_step_amp(float* const* params, float* const* grads, float* exp_avg, float* exp_avg_sq,
@@ -579,8 +583,8 @@ int snb_optim_step_amp(float* const* params, float* const* grads, float* exp_avg
   if (int rc = check_optim_step(who, params, reinterpret_cast<const void* const*>(grads), exp_avg, exp_avg_sq,
                                 slow_buffer, args, amp->base, precision, packed))
     return rc;
-  return optim_step_pack_amp(params, grads, exp_avg, exp_avg_sq, slow_buffer, *args, *amp, precision, new_activation,
-                             packed, reinterpret_cast<cudaStream_t>(stream));
+  return fused_step(SNB_N_PARAM_TENSORS, nullptr, params, grads, false, amp->base, amp, exp_avg, exp_avg_sq,
+                    slow_buffer, *args, precision, new_activation, packed, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_optim_step_tensors(int n, float* const* params, const float* const* grads, const int64_t* numel,
@@ -589,8 +593,8 @@ int snb_optim_step_tensors(int n, float* const* params, const float* const* grad
   if (int rc = check_optim_tensors("snb_optim_step_tensors", n, params, reinterpret_cast<const void* const*>(grads),
                                    numel, step, exp_avg, exp_avg_sq, slow_buffer, args))
     return rc;
-  return optim_step_tensors(n, params, grads, numel, step, exp_avg, exp_avg_sq, slow_buffer, *args,
-                            reinterpret_cast<cudaStream_t>(stream));
+  return fused_step(n, numel, params, grads, false, step, nullptr, exp_avg, exp_avg_sq, slow_buffer, *args, 0, 0,
+                    nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_optim_step_tensors_amp(int n, float* const* params, float* const* grads, const int64_t* numel,
@@ -601,8 +605,8 @@ int snb_optim_step_tensors_amp(int n, float* const* params, float* const* grads,
   if (int rc = check_optim_tensors(who, n, params, reinterpret_cast<const void* const*>(grads), numel, amp->base,
                                    exp_avg, exp_avg_sq, slow_buffer, args))
     return rc;
-  return optim_step_tensors_amp(n, params, grads, numel, exp_avg, exp_avg_sq, slow_buffer, *args, *amp,
-                                reinterpret_cast<cudaStream_t>(stream));
+  return fused_step(n, numel, params, grads, false, amp->base, amp, exp_avg, exp_avg_sq, slow_buffer, *args, 0, 0,
+                    nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int snb_depth_smooth_forward(const float* idepth, const int64_t* idepth_strides, const float* image,

@@ -99,8 +99,8 @@ int launch_pack_tc(const float* const* params, int precision, int new_activation
                    cudaStream_t st);
 
 // One term of the checksum: the 32-bit word of the parameter at flat index `idx` over the 24 concatenated tensors,
-// mixed with its position.  params_check_kernel and adam_step_kernel both sum these and must agree bit for bit:
-// otherwise every pass after an optimiser step sees a stale checksum and re-packs the image.
+// mixed with its position.  params_check_kernel and the optimiser's step_kernel both sum these and must agree bit for
+// bit: otherwise every pass after an optimiser step sees a stale checksum and re-packs the image.
 __device__ __forceinline__ unsigned long long param_checksum_term(unsigned long long idx, uint32_t word) {
   unsigned long long x = (idx << 32) ^ (unsigned long long)word ^ 0x9e3779b97f4a7c15ull;
   x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;

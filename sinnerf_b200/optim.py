@@ -165,13 +165,14 @@ def _amp_tensor(t, dev):
 
 
 class _FusedPerTensor(torch.optim.Optimizer):
-    """Shared body of FusedSGD / FusedRAdam / FusedRanger (C ABI snb_optim_step): one kernel per model and step, then
-    the re-pack of the weight image on the same stream.  For Discriminator modules (and FusedAdam over them): one
+    """Shared body of the four fused optimisers: one kernel per model and step, then the re-pack of the weight image on
+    the same stream (C ABI snb_optim_step; FusedAdam: snb_adam_step).  For Discriminator modules: one
     snb_optim_step_tensors launch per module and step, nothing to re-pack.
 
     These rules keep a step count per parameter and skip parameters without a gradient, so the count is tracked per
-    tensor (`_counts`, one `_Counts` per module) and passed to the kernel per tensor.  State mirrors the reference's exactly: a parameter has a
-    `state` entry only once it has been stepped, holding views of the flat buffers the kernel updates."""
+    tensor (`_counts`, one `_Counts` per module) and passed to the kernel per tensor; FusedAdam over NeRF models keeps
+    torch.optim.Adam's one count instead.  State mirrors the reference's exactly: a parameter has a `state` entry only
+    once it has been stepped, holding views of the flat buffers the kernel updates."""
     _rule: int
     _buffers: tuple          # state keys of the flat buffers, in snb_optim_step's argument order
     _has_step: bool = True   # the state carries the reference's per-parameter `step`
@@ -183,14 +184,14 @@ class _FusedPerTensor(torch.optim.Optimizer):
         self._precision = precision
         if not amp_scaling:
             self._step_supports_amp_scaling = False
+        # FusedAdam over NeRF models: torch.optim.Adam's one step count per model, advanced by every step
+        self._one_count = self._rule == _lib.OPTIM_ADAM and not self._disc
         self._flat = []          # per model: the flat state buffers, in _buffers order
         self._views = {}         # parameter -> {state key: view of its slice of the flat buffer}
         self._slot = {}          # parameter -> (model index, tensor index): where its update count is kept
-        self._counts = [_Counts(self._n_counts(m)) for m in self.models]   # the reference's state['step'] per tensor
+        # the reference's state['step'] per tensor
+        self._counts = [_Counts(1 if self._one_count else len(_params(m))) for m in self.models]
         self._stale = False      # GradScaler-native steps ran since `state` was last published
-
-    def _n_counts(self, m) -> int:
-        return len(_params(m))
 
     @property
     def state(self):
@@ -292,48 +293,42 @@ class _FusedPerTensor(torch.optim.Optimizer):
         group = self.param_groups[0]
         args = self._args(group)
         adv = self._advances(group)
+        # the entry point: snb_optim_step_tensors (Discriminators), snb_adam_step (FusedAdam over NeRF models) or
+        # snb_optim_step, each in its plain and its GradScaler-native (_amp) form
+        entry = "snb_optim_step_tensors" if self._disc else "snb_adam_step" if self._one_count else "snb_optim_step"
+        n_bufs = 2 if self._one_count else 3
         amp_step = False
         for m, bufs, counts in zip(self.models, self._flat, self._counts):
             ps = _params(m)
             dev = ps[0].device
             _check_tensors(ps, type(self).__name__)
-            advances = [p.grad is not None and adv for p in ps]
+            advances = [True] if self._one_count else [p.grad is not None and adv for p in ps]
             parr = (C.c_void_p * len(ps))(*[p.data_ptr() for p in ps])
             garr = (C.c_void_p * len(ps))(*[(p.grad.data_ptr() if p.grad is not None else None) for p in ps])
-            st = [_lib.ptr(b) for b in bufs] + [None] * (3 - len(bufs))
-            amp = self._amp_inputs(dev)
-            if amp is not None:
-                amp_step = True
-                with torch.cuda.device(dev):
-                    ctl = self._amp_ctl(counts, advances, amp, dev)
-                    if self._disc:
-                        _lib.check(lib.snb_optim_step_tensors_amp(len(ps), parr, garr,
-                                                                  (C.c_int64 * len(ps))(*[p.numel() for p in ps]), *st,
-                                                                  C.byref(args), C.byref(ctl), _lib.stream_ptr(dev)),
-                                   "snb_optim_step_tensors_amp")
-                    else:
-                        prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
-                        image = m.packed_image_buffer(prec)
-                        _lib.check(lib.snb_optim_step_amp(parr, garr, *st, C.byref(args), C.byref(ctl), prec,
-                                                          int(m.use_new_activation), _lib.ptr(image),
-                                                          _lib.stream_ptr(dev)), "snb_optim_step_amp")
-                    counts.advance(advances)
-                continue
-            counts.settle()
-            counts.load([c + 1 if a else c for c, a in zip(counts.host, advances)])
-            with torch.cuda.device(dev):
-                if self._disc:
-                    _lib.check(lib.snb_optim_step_tensors(len(ps), parr, garr,
-                                                          (C.c_int64 * len(ps))(*[p.numel() for p in ps]),
-                                                          (C.c_int * len(ps))(*counts.host), *st,
-                                                          C.byref(args), _lib.stream_ptr(dev)), "snb_optim_step_tensors")
-                    continue
+            st = [_lib.ptr(b) for b in bufs] + [None] * (n_bufs - len(bufs))
+            if self._disc:
+                head, tail = [len(ps), parr, garr, (C.c_int64 * len(ps))(*[p.numel() for p in ps])], []
+            else:
                 prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
-                for i, c in enumerate(counts.host):
-                    args.step[i] = c
-                image = m.packed_image_buffer(prec)
-                _lib.check(lib.snb_optim_step(parr, garr, *st, C.byref(args), prec, int(m.use_new_activation),
-                                              _lib.ptr(image), _lib.stream_ptr(dev)), "snb_optim_step")
+                head, tail = [parr, garr], [prec, int(m.use_new_activation), _lib.ptr(m.packed_image_buffer(prec))]
+            amp = self._amp_inputs(dev)
+            with torch.cuda.device(dev):
+                if amp is not None:
+                    amp_step = True
+                    ctl = self._amp_ctl(counts, advances, amp, dev)
+                    _lib.check(getattr(lib, entry + "_amp")(*head, *st, C.byref(args), C.byref(ctl), *tail,
+                                                            _lib.stream_ptr(dev)), entry + "_amp")
+                    counts.advance(advances)
+                    continue
+                counts.settle()
+                counts.load([c + 1 if a else c for c, a in zip(counts.host, advances)])
+                if self._disc:
+                    head.append((C.c_int * len(ps))(*counts.host))
+                elif self._one_count:
+                    args.step = counts.host[0]
+                else:
+                    args.step[:len(ps)] = counts.host
+                _lib.check(getattr(lib, entry)(*head, *st, C.byref(args), *tail, _lib.stream_ptr(dev)), entry)
         if amp_step:
             self._stale = True
         else:
@@ -364,9 +359,6 @@ class FusedAdam(_FusedPerTensor):
                  weight_decay: float = 0.0, precision: Optional[str] = None, amp_scaling: bool = True):
         super().__init__(models, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), precision, amp_scaling)
 
-    def _n_counts(self, m):
-        return len(_params(m)) if self._disc else 1
-
     @property
     def _steps(self) -> int:
         """NeRF models: updates applied so far (one count per model; all models step together)."""
@@ -382,6 +374,9 @@ class FusedAdam(_FusedPerTensor):
             st["step"] = torch.tensor(float(self._steps))
 
     def _args(self, group):
+        if self._one_count:
+            return _lib.SnbAdamArgs(float(group["lr"]), float(group["betas"][0]), float(group["betas"][1]),
+                                    float(group["eps"]), float(group["weight_decay"]), 0)
         return _lib.SnbOptimArgs(rule=self._rule, lr=float(group["lr"]), weight_decay=float(group["weight_decay"]),
                                  beta1=float(group["betas"][0]), beta2=float(group["betas"][1]), eps=float(group["eps"]),
                                  k=1)
@@ -425,50 +420,6 @@ class FusedAdam(_FusedPerTensor):
             step = max(step, int(float(st.get("step", 0))))
         for c in self._counts:
             c.load([step])
-
-    @torch.no_grad()
-    def step(self, closure=None):
-        if self._disc:
-            return super().step(closure)
-        loss = None
-        if closure is not None:
-            with torch.enable_grad():
-                loss = closure()
-        self._ensure_state()
-        lib = _lib.load()
-        g = self.param_groups[0]
-        amp_step = False
-        args = _lib.SnbAdamArgs(float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]),
-                                float(g["weight_decay"]), 0)
-        for m, (ea, es), counts in zip(self.models, self._flat, self._counts):
-            prec = config.step_precision(self._precision, getattr(m, "_last_prec", None))
-            ps = m._param_list()
-            dev = ps[0].device
-            _check_tensors(ps, "FusedAdam")
-            image = m.packed_image_buffer(prec)
-            parr = (C.c_void_p * 24)(*[p.data_ptr() for p in ps])
-            garr = (C.c_void_p * 24)(*[(p.grad.data_ptr() if p.grad is not None else None) for p in ps])
-            amp = self._amp_inputs(dev)
-            with torch.cuda.device(dev):
-                if amp is not None:
-                    amp_step = True
-                    ctl = self._amp_ctl(counts, [True], amp, dev)
-                    _lib.check(lib.snb_adam_step_amp(parr, garr, _lib.ptr(ea), _lib.ptr(es), C.byref(args),
-                                                     C.byref(ctl), prec, int(m.use_new_activation), _lib.ptr(image),
-                                                     _lib.stream_ptr(dev)), "snb_adam_step_amp")
-                    counts.advance([True])
-                    continue
-                counts.settle()
-                counts.load([counts.host[0] + 1])
-                args.step = counts.host[0]
-                _lib.check(lib.snb_adam_step(parr, garr, _lib.ptr(ea), _lib.ptr(es), C.byref(args), prec,
-                                             int(m.use_new_activation), _lib.ptr(image), _lib.stream_ptr(dev)),
-                           "snb_adam_step")
-        if amp_step:
-            self._stale = True
-        else:
-            self._publish()
-        return loss
 
 
 class FusedSGD(_FusedPerTensor):

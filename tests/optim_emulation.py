@@ -493,9 +493,8 @@ def measured_report():
 
 # ------------------------------------------------------------------------------------------------ checkers
 KERNELS = {
-    ("nerf", "adam"): "adam_step_kernel", ("nerf_amp", "adam"): "adam_step_amp_kernel",
-    ("nerf", "rule"): "optim_step_kernel<{}>", ("nerf_amp", "rule"): "optim_step_amp_kernel<{}>",
-    ("tensors", "rule"): "optim_tensors_kernel<{}>", ("tensors_amp", "rule"): "optim_tensors_amp_kernel<{}>",
+    ("nerf", "rule"): "step_kernel<{}> (NeRF)", ("nerf_amp", "rule"): "step_kernel<{}> (NeRF, _amp)",
+    ("tensors", "rule"): "step_kernel<{}> (table)", ("tensors_amp", "rule"): "step_kernel<{}> (table, _amp)",
 }
 
 

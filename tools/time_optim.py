@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""CUDA-event times of the optimiser step, fused against the rules it replaces (oracle/optim_oracle.py: the reference's
-SGD / RAdam / Ranger restated with torch ops, one ATen kernel per operation and tensor):
+"""CUDA-event times of the optimiser step, fused against the optimiser it replaces (torch.optim.Adam on its default
+foreach path; oracle/optim_oracle.py: the reference's SGD / RAdam / Ranger restated with torch ops, one ATen kernel per
+operation and tensor):
 
   1. one optimiser step over both NeRFs (48 tensors, 1.19 M parameters).  The fused step includes the re-pack of the
-     weight images; the oracle's step leaves them stale, and the next forward re-packs them (counted in 2.);
+     weight images; the replaced step leaves them stale, and the next forward re-packs them (counted in 2.);
   2. the tools/time_train.py training step (4 x 4096 rays, 64 + 64 samples, forward + backward) followed by the step.
 
     python tools/time_optim.py [--steps 50] [--iters 5] [--rays 4096] [--calls 4]
@@ -32,7 +33,10 @@ args = ap.parse_args()
 dev = torch.device("cuda:0")
 LR, WD = 5e-4, 0.0
 
-OPTIMIZERS = {   # name -> (fused, oracle) constructors with get_optimizer's arguments (reference utils/__init__.py:15-27)
+# name -> (fused, replaced) constructors with get_optimizer's arguments (reference utils/__init__.py:15-27)
+OPTIMIZERS = {
+    "adam": (lambda ms: FusedAdam(ms, lr=LR, eps=1e-8, weight_decay=WD),
+             lambda ps: torch.optim.Adam(ps, lr=LR, eps=1e-8, weight_decay=WD)),
     "sgd": (lambda ms: FusedSGD(ms, lr=LR, momentum=0.9, weight_decay=WD),
             lambda ps: optim_oracle.SGD(ps, lr=LR, momentum=0.9, weight_decay=WD)),
     "radam": (lambda ms: FusedRAdam(ms, lr=LR, eps=1e-8, weight_decay=WD),
@@ -72,15 +76,15 @@ print(f"device: {torch.cuda.get_device_name(dev)} | nvidia-smi: {gpu}")
 # ---- 1. the optimiser step alone (synthetic gradients of the training step's magnitude)
 print(f"\n1. one optimiser step over both models (mean of {args.steps} steps)")
 g = torch.Generator(device=dev).manual_seed(0)
-for name, (make_fused, make_oracle) in OPTIMIZERS.items():
+for name, (make_fused, make_replaced) in OPTIMIZERS.items():
     row = []
-    for impl in ("fused", "oracle"):
+    for impl in ("fused", "replaced"):
         ms = fresh_models()
         for p in (p for m in ms for p in m.parameters()):
             p.grad = torch.randn(p.shape, device=dev, generator=g) * 1e-3
-        opt = make_fused(ms) if impl == "fused" else make_oracle([p for m in ms for p in m.parameters()])
+        opt = make_fused(ms) if impl == "fused" else make_replaced([p for m in ms for p in m.parameters()])
         row.append(timed(opt.step, args.steps))
-    print(f"  {name:7s} fused {row[0]:7.3f} ms   oracle {row[1]:7.3f} ms   ({row[1] / row[0]:.1f}x)")
+    print(f"  {name:7s} fused {row[0]:7.3f} ms   replaced {row[1]:7.3f} ms   ({row[1] / row[0]:.1f}x)")
 
 # ---- 2. the training step of tools/time_train.py followed by the optimiser step
 print(f"\n2. training step ({args.calls} x {args.rays} rays, 64+64 samples, fwd + bwd) + optimiser step "
@@ -102,10 +106,10 @@ def train_step(models, opt):
     opt.step()
 
 
-rows = [("adam", "fused", lambda ms: FusedAdam(ms, lr=LR, eps=1e-8, weight_decay=WD))]
-for name, (make_fused, make_oracle) in OPTIMIZERS.items():
+rows = []
+for name, (make_fused, make_replaced) in OPTIMIZERS.items():
     rows.append((name, "fused", make_fused))
-    rows.append((name, "oracle", lambda ms, mk=make_oracle: mk([p for m in ms for p in m.parameters()])))
+    rows.append((name, "replaced", lambda ms, mk=make_replaced: mk([p for m in ms for p in m.parameters()])))
 for name, impl, make in rows:
     ms = fresh_models()
     opt = make(ms)
