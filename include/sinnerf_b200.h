@@ -422,6 +422,25 @@ int snb_disc_backward(int imsize, int precision, const float* const* weights, in
                       const float* d_out, float* d_input, const int64_t* d_strides, float* const* d_weights,
                       void* workspace, void* stream);
 
+/* Gradient penalty (models/sinnerf.py compute_grad2 for one output): snb_disc_penalty_forward is snb_disc_forward
+ * (same arguments, checks, output bits and u / v update) followed by g = d(sum out) / d input through the first-order
+ * chain and reg[b] = sum over image b of g^2 (reg: n floats, device).  g and everything the backward needs stay in
+ * the workspace: snb_disc_penalty_workspace_bytes(imsize, n, height, width) bytes (0 for a shape the forward
+ * refuses).  snb_disc_penalty_backward gives the gradients of <d_out, out> + <d_reg, reg> with respect to the input
+ * (d_input NULL: not wanted; written through d_strides) and to each weight_orig (NULL entries not wanted), with the
+ * forward's sigma, u and v: the first-order part exactly as snb_disc_backward computes it, plus the second-order
+ * part of the penalty (through sigma as spectral_norm differentiates it).  d_out (n, 1, oh, ow) or d_reg (n,), both
+ * contiguous, may be NULL (no such term), not both.  Every wanted element is written, not accumulated.  Neither call
+ * synchronises with the host; the workspace's saved part is only read by the backward. */
+size_t snb_disc_penalty_workspace_bytes(int imsize, int n, int height, int width);
+int snb_disc_penalty_forward(int imsize, int precision, int training, const float* const* weights,
+                             float* const* weight_u, float* const* weight_v, const float* input, const int64_t* strides,
+                             int n, int height, int width, const SnbDiscAug* aug, float* out, float* reg,
+                             void* workspace, void* stream);
+int snb_disc_penalty_backward(int imsize, int precision, const float* const* weights, int n, int height, int width,
+                              const float* d_out, const float* d_reg, float* d_input, const int64_t* d_strides,
+                              float* const* d_weights, void* workspace, void* stream);
+
 /* ---- optimiser step (SURVEY.md 8f-4) --------------------------------------------------------------
  * torch.optim.Adam as the reference configures it (utils/__init__.py:19-21: lr, eps = 1e-8, weight_decay;
  * betas default (0.9, 0.999), amsgrad off), fused over the 24 parameter tensors of one NeRF, followed on the

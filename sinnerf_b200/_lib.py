@@ -160,6 +160,12 @@ SIGNATURES = {
                                    C.POINTER(SnbDiscAug), c_f, c_f, c_f]),
     "snb_disc_backward": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, c_f, c_f,
                                     C.POINTER(C.c_int64), C.POINTER(C.c_void_p), c_f, c_f]),
+    "snb_disc_penalty_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "snb_disc_penalty_forward": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                           C.POINTER(C.c_void_p), c_f, C.POINTER(C.c_int64), C.c_int, C.c_int, C.c_int,
+                                           C.POINTER(SnbDiscAug), c_f, c_f, c_f, c_f]),
+    "snb_disc_penalty_backward": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, c_f,
+                                            c_f, c_f, C.POINTER(C.c_int64), C.POINTER(C.c_void_p), c_f, c_f]),
 }
 VIT_N_TENSORS = 148       # SNB_VIT_N_TENSORS
 VIT_MAX_IMAGES = 8        # SNB_VIT_MAX_IMAGES

@@ -24,6 +24,9 @@
 // gradient is written: the scaling is exact wherever that gradient is a normal float, and below that it is rounded
 // once (never flushed to zero by an intermediate factor).  Every reduction runs in a fixed order: two identical calls
 // give the same bits.
+// The gradient penalty of dloss='wgan_gp' (snb_disc_penalty_*, DESIGN §4.6) reuses this chain: g = grad_x sum(out)
+// is the backward from an all-ones upstream, and the penalty's second-order gradients are a tangent forward along
+// v = 2 d_reg g followed by a reverse pass over two adjoint streams, on the same GEMM and the same scaling rules.
 #include "common.cuh"
 #include "tc_gemm.cuh"
 
@@ -92,9 +95,16 @@ struct DiscWs {
   float* ws[kMaxLayers];          // 2^e W_orig, its largest element in [2^14, 2^15)
   float *col[kMaxLayers], *y[kMaxLayers], *mean[kMaxLayers], *rstd[kMaxLayers];
   float *dy0, *dy1, *dcol, *dx;   // backward scratch
+  // gradient penalty (pen = 1): g = grad_x sum(out) (n, 3, h, w), the tangent direction v, its DiffAugment
+  // parameters, each layer's tangent im2col and pre-norm tangent output with its InstanceNorm statistics, the
+  // primal-adjoint stream's scratch and both streams' raw weight gradients
+  float *g, *ones, *vt, *taug, *dp0, *dp1, *dcolp;
+  float *tcol[kMaxLayers], *ty[kMaxLayers], *tmean[kMaxLayers], *tq[kMaxLayers], *dwt[kMaxLayers], *dwp[kMaxLayers];
+  int *ev, *gt, *gp, *gu, *gw;    // per layer: exponents of the tangent col, of both adjoint streams, of a fold's
+                                  // primal output and of the combined weight gradient
   size_t bytes;
 };
-DiscWs disc_ws(void* base, const Net& N, int save) {
+DiscWs disc_ws(void* base, const Net& N, int save, int pen = 0) {
   DiscWs W{};
   float* b = static_cast<float*>(base);
   long long off = 0;
@@ -117,6 +127,22 @@ DiscWs disc_ws(void* base, const Net& N, int save) {
   if (save) {
     W.dy0 = take(dy_max); W.dy1 = take(dy_max); W.dcol = take(dcol_max);
     W.dx = take(3ll * N.n * N.h * N.w);
+  }
+  if (pen) {
+    const long long img = 3ll * N.n * N.h * N.w;
+    W.g = take(img); W.vt = take(img); W.ones = take((long long)N.n * N.l[N.n_layers - 1].P());
+    W.taug = take((long long)kAugFloats * N.n);
+    W.dp0 = take(dy_max); W.dp1 = take(dy_max); W.dcolp = take(dcol_max);
+    int* e = reinterpret_cast<int*>(take(5 * kMaxLayers));
+    W.ev = e; W.gt = e + kMaxLayers; W.gp = e + 2 * kMaxLayers; W.gu = e + 3 * kMaxLayers; W.gw = e + 4 * kMaxLayers;
+    for (int i = 0; i < N.n_layers; ++i) {
+      const Layer& y = N.l[i];
+      const long long rows = (long long)N.n * y.P();
+      W.tcol[i] = take(rows * y.K());
+      if (y.act) W.ty[i] = take(rows * y.cout);
+      if (y.in_norm) { W.tmean[i] = take((long long)y.cout * N.n); W.tq[i] = take((long long)y.cout * N.n); }
+      W.dwt[i] = take(y.cout * y.K()); W.dwp[i] = take(y.cout * y.K());
+    }
   }
   W.bytes = (size_t)off * 4;
   return W;
@@ -304,6 +330,29 @@ __global__ void disc_aug_params_kernel(const float* __restrict__ x, long long s_
   }
 }
 
+// DiffAugment is affine in its input; the parameters of its linear part for a tangent v (n, 3, h, w) contiguous:
+// the call's own, without the brightness shift and with the contrast mean taken over the saturated tangent
+__global__ void disc_aug_tangent_params_kernel(const float* __restrict__ v, int h, int w, const float* __restrict__ aug,
+                                               float* __restrict__ taug) {
+  __shared__ float red[32];
+  const int b = blockIdx.x, P = h * w;
+  const float* q = aug + (long long)kAugFloats * b;
+  float* p = taug + (long long)kAugFloats * b;
+  if (q[0] == 0.f) {
+    if (threadIdx.x == 0) p[0] = 0.f;
+    return;
+  }
+  float acc = 0.f;
+  for (int t = threadIdx.x; t < P; t += blockDim.x)
+    for (int c = 0; c < 3; ++c) acc += aug_saturated(v + 3ll * b * P + t, P, c, 0.f, q[2]);
+  acc = block_sum(acc, red);
+  if (threadIdx.x == 0) {
+    for (int k = 0; k < 9; ++k) p[k] = q[k];
+    p[1] = 0.f;
+    p[4] = acc / (3.f * P);
+  }
+}
+
 __device__ __forceinline__ bool aug_cut(const float* p, int y, int x) {
   return (float)y >= p[5] && (float)y <= p[6] && (float)x >= p[7] && (float)x <= p[8];
 }
@@ -317,8 +366,12 @@ struct GatherArgs {
   const float* aug;             // layer 1: DiffAugment parameters
   int n, hin, win, hout, wout, stride, pad, K;
   float* col;
+  const float* prim;            // kTangent: the source layer's primal pre-norm output (LeakyReLU slope mask)
 };
 
+// kTangent (layers 2..): src holds the source layer's normalised tangent, which passes the LeakyReLU with the
+// slope the primal input took
+template <bool kTangent = false>
 __global__ void disc_gather_kernel(const GatherArgs a) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long P = (long long)a.hout * a.wout;
@@ -339,6 +392,15 @@ __global__ void disc_gather_kernel(const GatherArgs a) {
       } else {
         v = __ldg(px + ci * a.s_c);
       }
+    } else if constexpr (kTangent) {
+      const long long o = b * a.s_b + ci * a.s_c + iy * a.s_y + ix * a.s_x;
+      v = __ldg(a.src + o);
+      float nv = __ldg(a.prim + o);
+      if (a.mean != nullptr) {
+        const int r = ci * a.n + b;
+        nv = (nv - a.mean[r]) * a.rstd[r];
+      }
+      if (!(nv > 0.f)) v *= kSlope;
     } else {
       v = __ldg(a.src + b * a.s_b + ci * a.s_c + iy * a.s_y + ix * a.s_x);
       if (a.mean != nullptr) {
@@ -381,6 +443,24 @@ struct FoldArgs {
   float* out;                   // (cin, n, hin win)
 };
 
+// input pixel (y, x) of channel ci, image b: the sum of the dcol entries of the (up to 2 x 2) output positions whose
+// window covers it
+__device__ __forceinline__ float fold_at(const float* dcol, int b, int ci, int y, int x, int hout, int wout,
+                                         int stride, int pad, int K) {
+  float g = 0.f;
+  for (int ky = 0; ky < 4; ++ky) {
+    const int ty = y + pad - ky;
+    if (ty < 0 || ty % stride != 0 || ty / stride >= hout) continue;
+    for (int kx = 0; kx < 4; ++kx) {
+      const int tx = x + pad - kx;
+      if (tx < 0 || tx % stride != 0 || tx / stride >= wout) continue;
+      const long long j = (long long)b * hout * wout + (ty / stride) * wout + tx / stride;
+      g += dcol[j * K + ci * 16 + ky * 4 + kx];
+    }
+  }
+  return g;
+}
+
 __global__ void disc_fold_kernel(const FoldArgs a) {
   __shared__ float red[32];
   const int r = blockIdx.x, ci = r / a.n, b = r % a.n;
@@ -391,17 +471,7 @@ __global__ void disc_fold_kernel(const FoldArgs a) {
   float sg = 0.f, sgn = 0.f;
   for (int p = threadIdx.x; p < P; p += blockDim.x) {
     const int y = p / a.win, x = p % a.win;
-    float g = 0.f;
-    for (int ky = 0; ky < 4; ++ky) {
-      const int ty = y + a.pad - ky;
-      if (ty < 0 || ty % a.stride != 0 || ty / a.stride >= a.hout) continue;
-      for (int kx = 0; kx < 4; ++kx) {
-        const int tx = x + a.pad - kx;
-        if (tx < 0 || tx % a.stride != 0 || tx / a.stride >= a.wout) continue;
-        const long long j = (long long)b * a.hout * a.wout + (ty / a.stride) * a.wout + tx / a.stride;
-        g += a.dcol[j * a.K + ci * 16 + ky * 4 + kx];
-      }
-    }
+    float g = fold_at(a.dcol, b, ci, y, x, a.hout, a.wout, a.stride, a.pad, a.K);
     if (yr != nullptr) {
       const float nv = (yr[p] - mu) * rs;
       if (!(nv > 0.f)) g *= kSlope;
@@ -413,6 +483,151 @@ __global__ void disc_fold_kernel(const FoldArgs a) {
   if (a.mean == nullptr) return;
   const float mg = block_sum(sg, red) / (float)P, mgn = block_sum(sgn, red) / (float)P;
   for (int p = threadIdx.x; p < P; p += blockDim.x) o[p] = rs * (o[p] - mg - (yr[p] - mu) * rs * mgn);
+}
+
+// ------------------------------------------------------------------ gradient penalty: tangent and second-order fold
+// One block per (channel, image) row of a layer with InstanceNorm: the tangent of z = (y - mean) rstd along the
+// tangent yd of y, zd = rstd (yd - mean(yd) - z q) with q = mean(z (yd - mean(yd))); mean(yd) and q are kept for the
+// second-order fold.
+__global__ void disc_in_tangent_kernel(const float* __restrict__ yd, const float* __restrict__ y,
+                                       const float* __restrict__ mean, const float* __restrict__ rstd, int P,
+                                       float* __restrict__ tmean, float* __restrict__ tq, float* __restrict__ zd) {
+  __shared__ float red[32];
+  const long long o = (long long)blockIdx.x * P;
+  const float mu = mean[blockIdx.x], rs = rstd[blockIdx.x];
+  float s = 0.f;
+  for (int p = threadIdx.x; p < P; p += blockDim.x) s += yd[o + p];
+  const float m = block_sum(s, red) / (float)P;
+  float q = 0.f;
+  for (int p = threadIdx.x; p < P; p += blockDim.x) q += (y[o + p] - mu) * rs * (yd[o + p] - m);
+  q = block_sum(q, red) / (float)P;
+  for (int p = threadIdx.x; p < P; p += blockDim.x) zd[o + p] = rs * (yd[o + p] - m - (y[o + p] - mu) * rs * q);
+  if (threadIdx.x == 0) {
+    tmean[blockIdx.x] = m;
+    tq[blockIdx.x] = q;
+  }
+}
+
+// The fold of both adjoint streams into layer i's input row (ci, b), then back through layer i - 1's LeakyReLU and
+// InstanceNorm.  With gt / gp the folded, slope-masked tangent / primal adjoints, z the primal normalised value,
+// yc = yd - mean(yd) the tangent, q = mean(z yc), a = mean(gt yc) and c = mean(gt z):
+//   tangent  out_t = rstd (gt - mean(gt) - z c)                       (the first-order InstanceNorm backward)
+//   primal   out_p = rstd (gp - mean(gp) - z mean(gp z))
+//                  + rstd^2 (-a z + 3 q c z - c yc - q (gt - mean(gt)))   (zd's dependence on y through z and rstd)
+// The two primal terms carry the exponents gp_in and gt_in + ev (the tangent's); the sum is written at the latter,
+// stored to *e_out.  dcol_p null: a zero primal adjoint (the top layer).  mean null (no InstanceNorm): the masked
+// folds pass through.
+struct Fold2Args {
+  const float *dcol_t, *dcol_p;
+  int n, cin, hin, win, hout, wout, stride, pad, K;
+  const float *y, *mean, *rstd, *yd, *tmean, *tq;
+  const int *gt_in, *gp_in, *ev;
+  int* e_out;
+  float *out_t, *out_p;
+};
+
+__global__ void disc_fold2_kernel(const Fold2Args a) {
+  __shared__ float red[32];
+  const int r = blockIdx.x, ci = r / a.n, b = r % a.n;
+  const int P = a.hin * a.win;
+  const long long o = (long long)r * P;
+  const bool in = a.mean != nullptr;
+  const float mu = in ? a.mean[r] : 0.f, rs = in ? a.rstd[r] : 1.f;
+  const float tm = in ? a.tmean[r] : 0.f, q = in ? a.tq[r] : 0.f;
+  float st = 0.f, stz = 0.f, sp = 0.f, spz = 0.f, sa = 0.f;
+  for (int p = threadIdx.x; p < P; p += blockDim.x) {
+    const int y = p / a.win, x = p % a.win;
+    float gt = fold_at(a.dcol_t, b, ci, y, x, a.hout, a.wout, a.stride, a.pad, a.K);
+    float gp = a.dcol_p != nullptr ? fold_at(a.dcol_p, b, ci, y, x, a.hout, a.wout, a.stride, a.pad, a.K) : 0.f;
+    const float z = (a.y[o + p] - mu) * rs;
+    if (!(z > 0.f)) {
+      gt *= kSlope;
+      gp *= kSlope;
+    }
+    if (in) {
+      st += gt; stz += gt * z; sp += gp; spz += gp * z;
+      sa += gt * (a.yd[o + p] - tm);
+    }
+    a.out_t[o + p] = gt;
+    a.out_p[o + p] = gp;
+  }
+  const int eg = a.gp_in != nullptr ? *a.gp_in : 0;
+  if (!in) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) *a.e_out = eg;
+    return;
+  }
+  const float mt = block_sum(st, red) / (float)P, c = block_sum(stz, red) / (float)P;
+  const float mp = block_sum(sp, red) / (float)P, cp = block_sum(spz, red) / (float)P;
+  const float am = block_sum(sa, red) / (float)P;
+  const int ex = *a.gt_in + *a.ev;
+  for (int p = threadIdx.x; p < P; p += blockDim.x) {
+    const float z = (a.y[o + p] - mu) * rs, gt = a.out_t[o + p], gp = a.out_p[o + p];
+    const float cross = rs * rs * (-am * z + 3.f * q * c * z - c * (a.yd[o + p] - tm) - q * (gt - mt));
+    a.out_t[o + p] = rs * (gt - mt - z * c);
+    a.out_p[o + p] = ldexpf(rs * (gp - mp - z * cp), eg - ex) + cross;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) *a.e_out = ex;
+}
+
+// v = 2 d_reg[b] g[b] (n, 3, h, w): the tangent direction whose Hessian-vector product is the penalty's gradient
+__global__ void disc_pen_dir_kernel(const float* __restrict__ g, const float* __restrict__ d_reg, long long per_image,
+                                    long long m, float* __restrict__ v) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) v[i] = 2.f * d_reg[i / per_image] * g[i];
+}
+
+__global__ void disc_fill_kernel(float* __restrict__ x, long long m, float v) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) x[i] = v;
+}
+
+// reg[b] = sum g[b]^2, one block per image
+__global__ void disc_pen_reg_kernel(const float* __restrict__ g, long long per_image, float* __restrict__ reg) {
+  __shared__ float red[32];
+  const float* gb = g + blockIdx.x * per_image;
+  float s = 0.f;
+  for (long long i = threadIdx.x; i < per_image; i += blockDim.x) s += gb[i] * gb[i];
+  s = block_sum(s, red);
+  if (threadIdx.x == 0) reg[blockIdx.x] = s;
+}
+
+// the raw second-order weight gradient of each layer: dwt 2^(gt + ev) + dwp 2^gp, written to dwt at the larger
+// exponent (stored to gw); dwp null: no primal part (the top layer)
+struct CombArgs {
+  float* dwt[kMaxLayers];
+  const float* dwp[kMaxLayers];
+  int numel[kMaxLayers];
+  const int *gt, *gp, *ev;
+  int* gw;
+};
+
+__global__ void disc_pen_combine_kernel(const CombArgs a) {
+  const int l = blockIdx.y;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (a.dwt[l] == nullptr) return;
+  const int et = a.gt[l] + a.ev[l];
+  const int ep = a.dwp[l] != nullptr ? a.gp[l] : et;
+  const int e = et > ep ? et : ep;
+  if (i == 0) a.gw[l] = e;
+  if (i >= a.numel[l]) return;
+  float v = ldexpf(a.dwt[l][i], et - e);
+  if (a.dwp[l] != nullptr) v += ldexpf(a.dwp[l][i], ep - e);
+  a.dwt[l][i] = v;
+}
+
+// out[l] = src[l] (kAcc: out[l] += src[l])
+struct AddArgs {
+  float* out[kMaxLayers];
+  const float* src[kMaxLayers];
+  int numel[kMaxLayers];
+};
+
+template <bool kAcc>
+__global__ void disc_pen_add_kernel(const AddArgs a) {
+  const int l = blockIdx.y;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (a.out[l] == nullptr || i >= a.numel[l]) return;
+  a.out[l][i] = kAcc ? a.out[l][i] + a.src[l][i] : a.src[l][i];
 }
 
 // ------------------------------------------------------------------ gradient scale and DiffAugment backward
@@ -430,7 +645,8 @@ __global__ void disc_grad_scale_kernel(const float* g, long long m, float* dy, c
   if (threadIdx.x == 0) *e_out = (e_in != nullptr ? *e_in : 0) - k;
 }
 
-// one block per image: dx (3, n, h w) -> the input gradient through d_strides, unscaled
+// one block per image: dx (3, n, h w) -> the input gradient through d_strides, unscaled (kAcc: added to it)
+template <bool kAcc = false>
 __global__ void disc_aug_bwd_kernel(const float* __restrict__ dx, const float* __restrict__ aug, int n, int h, int w,
                                     const int* __restrict__ gexp, float* __restrict__ out, long long s_b,
                                     long long s_c, long long s_y, long long s_x) {
@@ -457,7 +673,10 @@ __global__ void disc_aug_bwd_kernel(const float* __restrict__ dx, const float* _
       const float m = (g[0] + g[1] + g[2]) / 3.f;
       for (int c = 0; c < 3; ++c) g[c] = sat * g[c] + (1.f - sat) * m;
     }
-    for (int c = 0; c < 3; ++c) out[b * s_b + c * s_c + y * s_y + x * s_x] = ldexpf(g[c], e);
+    for (int c = 0; c < 3; ++c) {
+      float* o = out + b * s_b + c * s_c + y * s_y + x * s_x;
+      *o = kAcc ? *o + ldexpf(g[c], e) : ldexpf(g[c], e);
+    }
   }
 }
 
@@ -656,9 +875,206 @@ int disc_backward_impl(const Net& N, const float* const* W, const float* d_out, 
   return SNB_OK;
 }
 
+// The forward, then g = grad_x sum(out) through the first-order chain (kept in the workspace) and reg[b] = |g[b]|^2.
+template <int kMode>
+int disc_penalty_forward_impl(const Net& N, const float* const* W, float* const* u_mod, float* const* v_mod,
+                              const float* x, const int64_t* xs, const AugIn& aug, int training, float* out, float* reg,
+                              const DiscWs& ws, cudaStream_t st) {
+  DISC_TRY(disc_forward_impl<kMode>(N, W, u_mod, v_mod, x, xs, aug, training, out, ws, st));
+  const long long n_out = (long long)N.n * N.l[N.n_layers - 1].P(), per_image = 3ll * N.h * N.w;
+  disc_fill_kernel<<<blocks_of(n_out, 256), 256, 0, st>>>(ws.ones, n_out, 1.f);
+  DISC_TRY(check_launch("disc_fill_kernel"));
+  const int64_t gs[4] = {per_image, (int64_t)N.h * N.w, N.w, 1};
+  float* none[kMaxLayers] = {};
+  DISC_TRY(disc_backward_impl<kMode>(N, W, ws.ones, ws.g, gs, none, ws, st));
+  disc_pen_reg_kernel<<<N.n, 256, 0, st>>>(ws.g, per_image, reg);
+  return check_launch("disc_pen_reg_kernel");
+}
+
+// The first-order gradients from d_out (disc_backward_impl), then the penalty's: for v = 2 d_reg g, the gradients of
+// sum(J_x out . v), by a tangent forward along v and a reverse pass over two adjoint streams (the tangent's, which
+// starts at 1 on every output, and the primal's, which starts at 0 and is fed by the InstanceNorm cross terms).
+template <int kMode>
+int disc_penalty_backward_impl(const Net& N, const float* const* W, const float* d_out, const float* d_reg,
+                               float* d_input, const int64_t* ds, float* const* d_weights, const DiscWs& ws,
+                               cudaStream_t st) {
+  const int L = N.n_layers;
+  const bool first = d_out != nullptr;
+  if (first) DISC_TRY(disc_backward_impl<kMode>(N, W, d_out, d_input, ds, d_weights, ws, st));
+  if (d_reg == nullptr) return SNB_OK;
+  // lowest layer whose input gradient is needed; stop = L with only the last weight wanted still runs that wgrad
+  bool any = d_input != nullptr;
+  int stop = d_input != nullptr ? 0 : L;
+  for (int i = 0; i < L; ++i) {
+    any = any || d_weights[i] != nullptr;
+    if (d_weights[i] != nullptr && stop == L) stop = i + 1;
+  }
+  if (!any) return SNB_OK;
+  const long long img = 3ll * N.n * N.h * N.w, P0 = (long long)N.h * N.w;
+  // tangent forward along v, each layer's tangent col scaled to [2^14, 2^15) with its exponent in ev
+  disc_pen_dir_kernel<<<blocks_of(img, 256), 256, 0, st>>>(ws.g, d_reg, 3 * P0, img, ws.vt);
+  DISC_TRY(check_launch("disc_pen_dir_kernel"));
+  disc_grad_scale_kernel<<<1, 1024, 0, st>>>(ws.vt, img, ws.vt, nullptr, ws.ev);
+  DISC_TRY(check_launch("disc_grad_scale_kernel"));
+  disc_aug_tangent_params_kernel<<<N.n, 256, 0, st>>>(ws.vt, N.h, N.w, ws.aug, ws.taug);
+  DISC_TRY(check_launch("disc_aug_tangent_params_kernel"));
+  float* zd = ws.dy0;
+  for (int i = 0; i < L; ++i) {
+    const Layer& y = N.l[i];
+    const long long rows = (long long)N.n * y.P();
+    GatherArgs g{};
+    if (i == 0) {
+      g.src = ws.vt; g.s_b = 3 * P0; g.s_c = P0; g.s_y = N.w; g.s_x = 1;
+      g.aug = ws.taug;
+    } else {
+      const Layer& p = N.l[i - 1];
+      g.src = zd; g.prim = ws.y[i - 1]; g.s_b = p.P(); g.s_c = N.n * p.P(); g.s_y = p.wout; g.s_x = 1;
+      g.mean = ws.mean[i - 1]; g.rstd = ws.rstd[i - 1];
+    }
+    g.n = N.n; g.hin = y.hin; g.win = y.win; g.hout = y.hout; g.wout = y.wout; g.stride = y.stride; g.pad = y.pad;
+    g.K = (int)y.K(); g.col = ws.tcol[i]; g.scale = 1.f;
+    if (i == 0) disc_gather_kernel<<<blocks_of(rows * y.K(), 256), 256, 0, st>>>(g);
+    else disc_gather_kernel<true><<<blocks_of(rows * y.K(), 256), 256, 0, st>>>(g);
+    DISC_TRY(check_launch("disc_gather_kernel"));
+    if (i == L - 1) break;   // the penalty needs only the adjoint of the last tangent output (1 everywhere)
+    Gemm m = gemm(y.cout, (int)rows, (int)y.K());
+    m.A = ws.ws[i]; m.a_m = y.K(); m.a_k = 1;
+    m.Bf = ws.tcol[i]; m.b_n = y.K(); m.b_k = 1;
+    m.C = ws.ty[i]; m.c_m = rows;
+    m.alpha_dev = ws.alpha + i;
+    DISC_TRY((run_gemm<kMode, true>(m, 1, st)));
+    const float* zsrc = ws.ty[i];
+    if (y.in_norm) {
+      disc_in_tangent_kernel<<<y.cout * N.n, 256, 0, st>>>(ws.ty[i], ws.y[i], ws.mean[i], ws.rstd[i], (int)y.P(),
+                                                            ws.tmean[i], ws.tq[i], zd);
+      DISC_TRY(check_launch("disc_in_tangent_kernel"));
+      zsrc = zd;
+    }
+    disc_grad_scale_kernel<<<1, 1024, 0, st>>>(zsrc, rows * y.cout, zd, ws.ev + i, ws.ev + i + 1);
+    DISC_TRY(check_launch("disc_grad_scale_kernel"));
+  }
+  // reverse: t = the tangent stream's adjoint (exponents gt), p = the primal stream's (exponents gp)
+  const Layer& last = N.l[L - 1];
+  float *t = ws.dy0, *t_next = ws.dy1, *p = ws.dp0, *p_next = ws.dp1;
+  disc_grad_scale_kernel<<<1, 1024, 0, st>>>(ws.ones, (long long)N.n * last.P(), t, nullptr, ws.gt + L - 1);
+  DISC_TRY(check_launch("disc_grad_scale_kernel"));
+  bool have_p = false;   // the primal adjoint of the top layer is zero
+  for (int i = L - 1; i >= 0; --i) {
+    const Layer& y = N.l[i];
+    const long long rows = (long long)N.n * y.P();
+    if (d_weights[i] != nullptr) {  // dW = t tcol^T (+ p col^T), each at its own exponent until combined
+      Gemm m = gemm(y.cout, (int)y.K(), (int)rows);
+      m.A = t; m.a_m = rows; m.a_k = 1;
+      m.Bf = ws.tcol[i]; m.b_n = 1; m.b_k = y.K();
+      m.C = ws.dwt[i]; m.c_m = y.K();
+      DISC_TRY(run_gemm<kMode>(m, 1, st));
+      if (have_p) {
+        m.A = p; m.Bf = ws.col[i]; m.C = ws.dwp[i];
+        m.alpha = 1.f / col_scale(N, i);
+        DISC_TRY(run_gemm<kMode>(m, 1, st));
+      }
+    }
+    if (i < stop) break;
+    {  // dcol = (1 / sigma) W^T [t p]: both streams in one launch, as two matrices along z
+      Gemm m = gemm((int)rows, (int)y.K(), y.cout);
+      m.A = t; m.a_m = 1; m.a_k = rows; m.a_z1 = p - t;
+      m.Bf = ws.ws[i]; m.b_n = 1; m.b_k = y.K();
+      m.C = ws.dcol; m.c_m = y.K(); m.c_z1 = ws.dcolp - ws.dcol;
+      m.alpha_dev = ws.alpha + i;
+      if (i == 0) {   // only the primal stream reaches the input
+        m.A = p; m.C = ws.dcolp;
+      }
+      DISC_TRY((run_gemm<kMode, true>(m, i > 0 && have_p ? 2 : 1, st)));
+    }
+    if (i > 0) {
+      const int q = i - 1;
+      Fold2Args f{};
+      f.dcol_t = ws.dcol; f.dcol_p = have_p ? ws.dcolp : nullptr;
+      f.n = N.n; f.cin = y.cin; f.hin = y.hin; f.win = y.win; f.hout = y.hout; f.wout = y.wout;
+      f.stride = y.stride; f.pad = y.pad; f.K = (int)y.K();
+      f.y = ws.y[q]; f.mean = ws.mean[q]; f.rstd = ws.rstd[q]; f.yd = ws.ty[q]; f.tmean = ws.tmean[q]; f.tq = ws.tq[q];
+      f.gt_in = ws.gt + i; f.gp_in = have_p ? ws.gp + i : nullptr; f.ev = ws.ev + q; f.e_out = ws.gu + q;
+      f.out_t = t_next; f.out_p = p_next;
+      disc_fold2_kernel<<<y.cin * N.n, 256, 0, st>>>(f);
+      DISC_TRY(check_launch("disc_fold2_kernel"));
+      const long long m = (long long)y.cin * N.n * y.hin * y.win;
+      disc_grad_scale_kernel<<<1, 1024, 0, st>>>(t_next, m, t_next, ws.gt + i, ws.gt + q);
+      DISC_TRY(check_launch("disc_grad_scale_kernel"));
+      disc_grad_scale_kernel<<<1, 1024, 0, st>>>(p_next, m, p_next, ws.gu + q, ws.gp + q);
+      DISC_TRY(check_launch("disc_grad_scale_kernel"));
+      float* tmp = t; t = t_next; t_next = tmp;
+      tmp = p; p = p_next; p_next = tmp;
+      have_p = true;
+    } else {
+      FoldArgs f{};
+      f.dcol = ws.dcolp; f.n = N.n; f.cin = y.cin; f.hin = y.hin; f.win = y.win; f.hout = y.hout; f.wout = y.wout;
+      f.stride = y.stride; f.pad = y.pad; f.K = (int)y.K(); f.out = ws.dx;
+      disc_fold_kernel<<<y.cin * N.n, 256, 0, st>>>(f);
+      DISC_TRY(check_launch("disc_fold_kernel"));
+      if (first)
+        disc_aug_bwd_kernel<true><<<N.n, 256, 0, st>>>(ws.dx, ws.aug, N.n, N.h, N.w, ws.gp, d_input, ds[0], ds[1],
+                                                       ds[2], ds[3]);
+      else
+        disc_aug_bwd_kernel<<<N.n, 256, 0, st>>>(ws.dx, ws.aug, N.n, N.h, N.w, ws.gp, d_input, ds[0], ds[1], ds[2],
+                                                 ds[3]);
+      DISC_TRY(check_launch("disc_aug_bwd_kernel"));
+    }
+  }
+  // the weight gradients: combine the two streams, the spectral-norm correction, then add to (or write) the output
+  CombArgs c{};
+  FixArgs a{};
+  AddArgs d{};
+  long long most = 0;
+  for (int i = 0; i < L; ++i) {
+    const long long numel = N.l[i].cout * N.l[i].K();
+    const bool want = d_weights[i] != nullptr;
+    c.dwt[i] = want ? ws.dwt[i] : nullptr; c.dwp[i] = want && i < L - 1 ? ws.dwp[i] : nullptr; c.numel[i] = (int)numel;
+    a.dW[i] = c.dwt[i]; a.W[i] = W[i]; a.u[i] = ws.u[i]; a.v[i] = ws.v[i]; a.part[i] = ws.part[i];
+    a.rows[i] = N.l[i].cout; a.cols[i] = (int)N.l[i].K();
+    d.out[i] = d_weights[i]; d.src[i] = ws.dwt[i]; d.numel[i] = (int)numel;
+    if (want) most = most > numel ? most : numel;
+  }
+  if (most == 0) return SNB_OK;
+  c.gt = ws.gt; c.gp = ws.gp; c.ev = ws.ev; c.gw = ws.gw;
+  a.inv_sigma = ws.inv_sigma; a.gexp = ws.gw;
+  const dim3 grid(blocks_of(most, 256), L);
+  disc_pen_combine_kernel<<<grid, 256, 0, st>>>(c);
+  DISC_TRY(check_launch("disc_pen_combine_kernel"));
+  disc_sn_dot_kernel<<<dim3(512, L), 256, 0, st>>>(a);
+  DISC_TRY(check_launch("disc_sn_dot_kernel"));
+  disc_sn_fix_kernel<<<grid, 256, 0, st>>>(a);
+  DISC_TRY(check_launch("disc_sn_fix_kernel"));
+  if (first) disc_pen_add_kernel<true><<<grid, 256, 0, st>>>(d);
+  else disc_pen_add_kernel<false><<<grid, 256, 0, st>>>(d);
+  return check_launch("disc_pen_add_kernel");
+}
+
 int check_ptrs(const char* who, const void* const* p, int n, const char* what, bool allow_null) {
   SNB_REQUIRE(p != nullptr, "%s: null %s array", who, what);
   for (int i = 0; i < n; ++i) SNB_REQUIRE(allow_null || p[i] != nullptr, "%s: null %s pointer %d", who, what, i);
+  return SNB_OK;
+}
+
+// the checks of a forward call, shared by snb_disc_forward and snb_disc_penalty_forward
+int forward_args(const char* who, int imsize, int precision, const float* const* weights, float* const* weight_u,
+                 float* const* weight_v, const float* input, const int64_t* strides, int n, int height, int width,
+                 const SnbDiscAug* aug, const float* out, const void* workspace, Net& N, AugIn& in, int& mode) {
+  mode = mode_of(precision);
+  if (mode < 0) return fail(SNB_ERR_UNSUPPORTED, "%s: unknown precision %d", who, precision);
+  DISC_TRY(net_of(who, imsize, n, height, width, N));
+  DISC_TRY(check_ptrs(who, reinterpret_cast<const void* const*>(weights), N.n_layers, "weight", false));
+  DISC_TRY(check_ptrs(who, reinterpret_cast<const void* const*>(weight_u), N.n_layers, "weight_u", false));
+  DISC_TRY(check_ptrs(who, reinterpret_cast<const void* const*>(weight_v), N.n_layers, "weight_v", false));
+  SNB_REQUIRE(input != nullptr && strides != nullptr && out != nullptr && workspace != nullptr,
+              "%s: null input, strides, out or workspace", who);
+  in = AugIn{};
+  if (aug != nullptr && aug->brightness != nullptr) {
+    SNB_REQUIRE(aug->saturation != nullptr && aug->contrast != nullptr && aug->cutout_y != nullptr &&
+                    aug->cutout_x != nullptr, "%s: DiffAugment draws must all be given or brightness NULL", who);
+    in.bright = aug->brightness; in.sat = aug->saturation; in.con = aug->contrast;
+    in.cut_y = aug->cutout_y; in.cut_x = aug->cutout_x;
+    in.cut_h = (int)(height * 0.5 + 0.5); in.cut_w = (int)(width * 0.5 + 0.5);
+  }
   return SNB_OK;
 }
 
@@ -679,23 +1095,11 @@ int snb_disc_forward(int imsize, int precision, int training, const float* const
                      float* const* weight_v, const float* input, const int64_t* strides, int n, int height, int width,
                      const SnbDiscAug* aug, float* out, void* workspace, void* stream) {
   const char* who = "snb_disc_forward";
-  const int mode = mode_of(precision);
-  if (mode < 0) return fail(SNB_ERR_UNSUPPORTED, "%s: unknown precision %d", who, precision);
   Net N;
-  DISC_TRY(net_of(who, imsize, n, height, width, N));
-  DISC_TRY(check_ptrs(who, reinterpret_cast<const void* const*>(weights), N.n_layers, "weight", false));
-  DISC_TRY(check_ptrs(who, reinterpret_cast<const void* const*>(weight_u), N.n_layers, "weight_u", false));
-  DISC_TRY(check_ptrs(who, reinterpret_cast<const void* const*>(weight_v), N.n_layers, "weight_v", false));
-  SNB_REQUIRE(input != nullptr && strides != nullptr && out != nullptr && workspace != nullptr,
-              "%s: null input, strides, out or workspace", who);
   AugIn in{};
-  if (aug != nullptr && aug->brightness != nullptr) {
-    SNB_REQUIRE(aug->saturation != nullptr && aug->contrast != nullptr && aug->cutout_y != nullptr &&
-                    aug->cutout_x != nullptr, "%s: DiffAugment draws must all be given or brightness NULL", who);
-    in.bright = aug->brightness; in.sat = aug->saturation; in.con = aug->contrast;
-    in.cut_y = aug->cutout_y; in.cut_x = aug->cutout_x;
-    in.cut_h = (int)(height * 0.5 + 0.5); in.cut_w = (int)(width * 0.5 + 0.5);
-  }
+  int mode;
+  DISC_TRY(forward_args(who, imsize, precision, weights, weight_u, weight_v, input, strides, n, height, width, aug,
+                        out, workspace, N, in, mode));
   const DiscWs W = disc_ws(workspace, N, 0);
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int tr = training ? 1 : 0;
@@ -721,6 +1125,55 @@ int snb_disc_backward(int imsize, int precision, const float* const* weights, in
   if (mode == kSplit) return disc_backward_impl<kSplit>(N, weights, d_out, d_input, d_strides, d_weights, W, st);
   if (mode == kF16) return disc_backward_impl<kF16>(N, weights, d_out, d_input, d_strides, d_weights, W, st);
   return disc_backward_impl<kBf16>(N, weights, d_out, d_input, d_strides, d_weights, W, st);
+}
+
+size_t snb_disc_penalty_workspace_bytes(int imsize, int n, int height, int width) {
+  Net N;
+  if (net_of("snb_disc_penalty_workspace_bytes", imsize, n, height, width, N) != SNB_OK) return 0;
+  return disc_ws(nullptr, N, 1, 1).bytes;
+}
+
+int snb_disc_penalty_forward(int imsize, int precision, int training, const float* const* weights,
+                             float* const* weight_u, float* const* weight_v, const float* input, const int64_t* strides,
+                             int n, int height, int width, const SnbDiscAug* aug, float* out, float* reg,
+                             void* workspace, void* stream) {
+  const char* who = "snb_disc_penalty_forward";
+  Net N;
+  AugIn in{};
+  int mode;
+  DISC_TRY(forward_args(who, imsize, precision, weights, weight_u, weight_v, input, strides, n, height, width, aug,
+                        out, workspace, N, in, mode));
+  SNB_REQUIRE(reg != nullptr, "%s: null reg", who);
+  const DiscWs W = disc_ws(workspace, N, 1, 1);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int tr = training ? 1 : 0;
+  if (mode == kSplit)
+    return disc_penalty_forward_impl<kSplit>(N, weights, weight_u, weight_v, input, strides, in, tr, out, reg, W, st);
+  if (mode == kF16)
+    return disc_penalty_forward_impl<kF16>(N, weights, weight_u, weight_v, input, strides, in, tr, out, reg, W, st);
+  return disc_penalty_forward_impl<kBf16>(N, weights, weight_u, weight_v, input, strides, in, tr, out, reg, W, st);
+}
+
+int snb_disc_penalty_backward(int imsize, int precision, const float* const* weights, int n, int height, int width,
+                              const float* d_out, const float* d_reg, float* d_input, const int64_t* d_strides,
+                              float* const* d_weights, void* workspace, void* stream) {
+  const char* who = "snb_disc_penalty_backward";
+  const int mode = mode_of(precision);
+  if (mode < 0) return fail(SNB_ERR_UNSUPPORTED, "%s: unknown precision %d", who, precision);
+  Net N;
+  DISC_TRY(net_of(who, imsize, n, height, width, N));
+  DISC_TRY(check_ptrs(who, reinterpret_cast<const void* const*>(weights), N.n_layers, "weight", false));
+  DISC_TRY(check_ptrs(who, reinterpret_cast<const void* const*>(d_weights), N.n_layers, "d_weight", true));
+  SNB_REQUIRE((d_out != nullptr || d_reg != nullptr) && workspace != nullptr, "%s: null d_out and d_reg, or null "
+              "workspace", who);
+  SNB_REQUIRE(d_input == nullptr || d_strides != nullptr, "%s: d_input without d_strides", who);
+  const DiscWs W = disc_ws(workspace, N, 1, 1);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (mode == kSplit)
+    return disc_penalty_backward_impl<kSplit>(N, weights, d_out, d_reg, d_input, d_strides, d_weights, W, st);
+  if (mode == kF16)
+    return disc_penalty_backward_impl<kF16>(N, weights, d_out, d_reg, d_input, d_strides, d_weights, W, st);
+  return disc_penalty_backward_impl<kBf16>(N, weights, d_out, d_reg, d_input, d_strides, d_weights, W, st);
 }
 
 }  // extern "C"

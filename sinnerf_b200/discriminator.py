@@ -18,11 +18,13 @@ stored u and v are used.  Nothing synchronises with the host.
 
 Inputs are (B, 3, H, W) fp32 CUDA tensors read through their strides; the input gradient comes back with the input's
 strides.  Gradients flow to the input and to every weight_orig.  The backward is once-differentiable: back-propagating
-through it raises, and so does a gradient penalty that needs a second-order gradient (dloss='wgan_gp',
-compute_grad2(create_graph=True)).  The GEMM arithmetic follows `precision=` or the process setting
-(config.resolve_precision), as in sinnerf_b200.vit: the fp16 hi + lo three-product split by default, 'f16' / 'bf16'
-single products, and under 'autocast' fp16 autocast gives 'f16', the arithmetic of the reference's cuDNN
-convolutions under Lightning's precision=16.  There is no CPU path.
+through it raises, so compute_grad2(create_graph=True) on D(x) does too.  The gradient penalty of dloss='wgan_gp'
+comes instead from `forward_with_penalty(input)`, which returns D(input) and compute_grad2's per-image penalty of
+the same call, both differentiable to first order (the penalty's gradients are second-order in the discriminator).
+The GEMM arithmetic follows `precision=` or the process setting (config.resolve_precision), as in
+sinnerf_b200.vit: the fp16 hi + lo three-product split by default, 'f16' / 'bf16' single products, and under
+'autocast' fp16 autocast gives 'f16', the arithmetic of the reference's cuDNN convolutions under Lightning's
+precision=16.  There is no CPU path.
 """
 from __future__ import annotations
 
@@ -135,6 +137,49 @@ class _DiscFn(torch.autograd.Function):
         return (None, dx, *dws)
 
 
+class _PenaltyFn(torch.autograd.Function):
+    """(D(x), compute_grad2(D(x), x)) for one call; backward from either or both with this call's sigma, u and v"""
+
+    @staticmethod
+    def forward(ctx, cfg, x, *weights):
+        imsize, mode, training, save, us, vs, aug, out_hw = cfg
+        lib = _lib.load()
+        B, _, H, W = x.shape
+        dev = x.device
+        ws = torch.empty(lib.snb_disc_penalty_workspace_bytes(imsize, B, H, W), device=dev, dtype=torch.uint8)
+        out = torch.empty(B, 1, *out_hw, device=dev, dtype=torch.float32)
+        reg = torch.empty(B, device=dev, dtype=torch.float32)
+        a = None if aug is None else _lib.SnbDiscAug(*[t.data_ptr() for t in aug])
+        _lib.check(lib.snb_disc_penalty_forward(imsize, mode, int(training), _ptrs(weights), _ptrs(us), _ptrs(vs),
+                                                _lib.ptr(x), (C.c_int64 * 4)(*x.stride()), B, H, W,
+                                                None if a is None else C.byref(a), _lib.ptr(out), _lib.ptr(reg),
+                                                _lib.ptr(ws), _lib.stream_ptr(dev)), "snb_disc_penalty_forward")
+        ctx.set_materialize_grads(False)
+        if save:
+            ctx.save_for_backward(ws, x, *weights)
+            ctx.cfg = (imsize, mode)
+        return out, reg
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out, g_reg):
+        ws, x, *weights = ctx.saved_tensors
+        if g_out is None and g_reg is None:
+            return (None, None, *[None] * len(weights))
+        lib = _lib.load()
+        imsize, mode = ctx.cfg
+        g_out = None if g_out is None else g_out.detach().to(torch.float32).contiguous()
+        g_reg = None if g_reg is None else g_reg.detach().to(torch.float32).contiguous()
+        dx = torch.empty_like(x) if ctx.needs_input_grad[1] else None
+        dws = [torch.empty_like(w) if need else None for w, need in zip(weights, ctx.needs_input_grad[2:])]
+        B, _, H, W = x.shape
+        strides = None if dx is None else (C.c_int64 * 4)(*dx.stride())
+        _lib.check(lib.snb_disc_penalty_backward(imsize, mode, _ptrs(weights), B, H, W, _lib.ptr(g_out),
+                                                 _lib.ptr(g_reg), _lib.ptr(dx), strides, _ptrs(dws), _lib.ptr(ws),
+                                                 _lib.stream_ptr(x.device)), "snb_disc_penalty_backward")
+        return (None, dx, *dws)
+
+
 class Discriminator(nn.Module):
     """models/discriminator.py Discriminator(conditional=False, policy, ndf=64, imsize) on the library's kernels.
 
@@ -171,9 +216,8 @@ class Discriminator(nn.Module):
     def convs(self):
         return [m for m in self.main if isinstance(m, nn.Conv2d)]
 
-    def forward(self, input, y=None):
-        x = input
-        what = "Discriminator"
+    def _call_args(self, x, what):
+        """the input checks of a call, then its draws: (cfg prefix, weights)"""
         if not isinstance(x, torch.Tensor):
             raise TypeError(f"{what}: input is not a torch.Tensor (got {type(x)})")
         if x.dim() != 4 or x.shape[0] < 1 or x.shape[1] != 3:
@@ -193,4 +237,21 @@ class Discriminator(nn.Module):
         mode = resolve_precision(self.precision)
         save = torch.is_grad_enabled() and (x.requires_grad or any(w.requires_grad for w in weights))
         cfg = (self.imsize if self.imsize in (128, 64, 32) else -1, mode, self.training, save, us, vs, aug, out_hw)
-        return _DiscFn.apply(cfg, x, *weights)
+        return cfg, weights
+
+    def forward(self, input, y=None):
+        cfg, weights = self._call_args(input, "Discriminator")
+        return _DiscFn.apply(cfg, input, *weights)
+
+    def forward_with_penalty(self, input, y=None):
+        """(out, reg): out is D(input) -- the same draws, bits and weight_u / weight_v update -- and reg (B,) is
+        models/sinnerf.py's compute_grad2(out, input) for this call, reg[b] = sum (d sum(out) / d input[b])^2 through
+        DiffAugment and every spectral-norm layer with this call's sigma, u and v.  Both are differentiable to first
+        order: reg back-propagates to every weight_orig (through sigma, as spectral_norm does) and to the input when
+        it requires grad.  input need not require grad.  The wgan_gp discriminator step:
+
+            pred_real, reg_real = D.forward_with_penalty(real_patch)
+            loss_d += 10 * reg_real.mean()
+        """
+        cfg, weights = self._call_args(input, "Discriminator.forward_with_penalty")
+        return _PenaltyFn.apply(cfg, input, *weights)
