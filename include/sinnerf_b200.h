@@ -441,6 +441,45 @@ int snb_disc_penalty_backward(int imsize, int precision, const float* const* wei
                               const float* d_out, const float* d_reg, float* d_input, const int64_t* d_strides,
                               float* const* d_weights, void* workspace, void* stream);
 
+/* ---- standalone DiffAugment ---------------------------------------------------------------------------
+ * models/diff_aug.py DiffAugment(x, policy) after its gate, with the draws given: the ops of the policy applied in
+ * order to (n, channels, height, width) fp32 read through in_strides (HOST, 4: image, channel, row, column), written
+ * to out through out_strides (every element).  ops: HOST array of n_ops (0 .. SNB_DIFF_AUG_MAX_OPS) op codes:
+ *   COLOR: x + (brightness - 0.5); about the per-pixel channel mean, factor 2 saturation; about the per-image mean
+ *          over channels, rows and columns, factor contrast + 0.5
+ *   TRANSLATION: out[y][x] = in[y + translation_y][x + translation_x], zero where that falls outside the image
+ *   CUTOUT: zero rows clamp(cutout_y - ch/2 .. + ch - 1) x columns clamp(cutout_x - cw/2 .. + cw - 1),
+ *           ch = (int)(height / 2 + 0.5), cw likewise
+ * draws: device pointers, the k-th occurrence of an op in the policy reading row k of its (occurrences, n) arrays;
+ * NULL for an op the policy does not list.  translation_y / _x are the reference's translation_x / _y (its shift of
+ * dim 2 and of dim 3), drawn from [-(int)(height / 8 + 0.5), +] and [-(int)(width / 8 + 0.5), +].
+ * Where COLOR precedes CUTOUT directly, the values are those snb_disc_forward's first layer reads for the same
+ * draws, bit for bit.  workspace: n * SNB_DIFF_AUG_WS_FLOATS floats (device), any content.  Two launches, no host
+ * synchronisation; two identical calls give the same bits. */
+#define SNB_DIFF_AUG_MAX_OPS 8
+#define SNB_DIFF_AUG_WS_FLOATS 32
+#define SNB_DIFF_AUG_COLOR 0
+#define SNB_DIFF_AUG_TRANSLATION 1
+#define SNB_DIFF_AUG_CUTOUT 2
+typedef struct SnbDiffAugDraws {
+  const float* brightness;        /* torch.rand draws */
+  const float* saturation;
+  const float* contrast;
+  const int64_t* translation_y;   /* torch.randint row shifts */
+  const int64_t* translation_x;   /* ... column shifts */
+  const int64_t* cutout_y;        /* torch.randint offsets along the rows */
+  const int64_t* cutout_x;        /* ... along the columns */
+} SnbDiffAugDraws;
+int snb_diff_augment_forward(const int* ops, int n_ops, const SnbDiffAugDraws* draws, const float* input,
+                             const int64_t* in_strides, int n, int channels, int height, int width, float* out,
+                             const int64_t* out_strides, float* workspace, void* stream);
+/* The input gradient of that map (it is affine in the input): d_out read through d_out_strides -> d_input written
+ * through d_in_strides, every element, nothing accumulated.  The same ops, draws and shapes as the forward; the
+ * input itself is not needed.  Two launches, no atomics, no host synchronisation. */
+int snb_diff_augment_backward(const int* ops, int n_ops, const SnbDiffAugDraws* draws, const float* d_out,
+                              const int64_t* d_out_strides, int n, int channels, int height, int width, float* d_input,
+                              const int64_t* d_in_strides, float* workspace, void* stream);
+
 /* ---- optimiser step (SURVEY.md 8f-4) --------------------------------------------------------------
  * torch.optim.Adam as the reference configures it (utils/__init__.py:19-21: lr, eps = 1e-8, weight_decay;
  * betas default (0.9, 0.999), amsgrad off), fused over the 24 parameter tensors of one NeRF, followed on the

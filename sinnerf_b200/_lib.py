@@ -77,6 +77,16 @@ class SnbDiscAug(C.Structure):
 
 DISC_MAX_LAYERS = 6   # SNB_DISC_MAX_LAYERS
 
+
+class SnbDiffAugDraws(C.Structure):
+    _fields_ = [("brightness", c_f), ("saturation", c_f), ("contrast", c_f), ("translation_y", c_f),
+                ("translation_x", c_f), ("cutout_y", c_f), ("cutout_x", c_f)]
+
+
+DIFF_AUG_MAX_OPS = 8       # SNB_DIFF_AUG_MAX_OPS
+DIFF_AUG_WS_FLOATS = 32    # SNB_DIFF_AUG_WS_FLOATS
+DIFF_AUG_OPS = {"color": 0, "translation": 1, "cutout": 2}   # SNB_DIFF_AUG_*
+
 LOSS_WS_FLOATS = 4096   # SNB_LOSS_WS_FLOATS
 PARAM_FLOATS = 595844   # SNB_PARAM_FLOATS
 
@@ -166,6 +176,12 @@ SIGNATURES = {
                                            C.POINTER(SnbDiscAug), c_f, c_f, c_f, c_f]),
     "snb_disc_penalty_backward": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, c_f,
                                             c_f, c_f, C.POINTER(C.c_int64), C.POINTER(C.c_void_p), c_f, c_f]),
+    "snb_diff_augment_forward": (C.c_int, [C.POINTER(C.c_int), C.c_int, C.POINTER(SnbDiffAugDraws), c_f,
+                                           C.POINTER(C.c_int64), C.c_int, C.c_int, C.c_int, C.c_int, c_f,
+                                           C.POINTER(C.c_int64), c_f, c_f]),
+    "snb_diff_augment_backward": (C.c_int, [C.POINTER(C.c_int), C.c_int, C.POINTER(SnbDiffAugDraws), c_f,
+                                            C.POINTER(C.c_int64), C.c_int, C.c_int, C.c_int, C.c_int, c_f,
+                                            C.POINTER(C.c_int64), c_f, c_f]),
 }
 VIT_N_TENSORS = 148       # SNB_VIT_N_TENSORS
 VIT_MAX_IMAGES = 8        # SNB_VIT_MAX_IMAGES

@@ -115,6 +115,37 @@ static int check_precision(int precision) {
   return SNB_OK;
 }
 
+// standalone DiffAugment (disc.cu)
+int launch_diff_augment(bool, const int*, int, const SnbDiffAugDraws&, const float*, const int64_t*, int, int, int, int,
+                        float*, const int64_t*, float*, cudaStream_t);
+
+// the checks of snb_diff_augment_forward / _backward
+static int check_diff_augment(const char* who, const int* ops, int n_ops, const SnbDiffAugDraws* d, const void* src,
+                              const int64_t* ss, int n, int channels, int height, int width, const void* dst,
+                              const int64_t* ds, const void* workspace) {
+  SNB_REQUIRE(n_ops >= 0 && n_ops <= SNB_DIFF_AUG_MAX_OPS, "%s: n_ops %d outside 0..%d", who, n_ops,
+              SNB_DIFF_AUG_MAX_OPS);
+  SNB_REQUIRE(n_ops == 0 || (ops != nullptr && d != nullptr), "%s: null ops or draws", who);
+  for (int k = 0; k < n_ops; ++k) {
+    const int op = ops[k];
+    SNB_REQUIRE(op == SNB_DIFF_AUG_COLOR || op == SNB_DIFF_AUG_TRANSLATION || op == SNB_DIFF_AUG_CUTOUT,
+                "%s: unknown op code %d at %d", who, op, k);
+    SNB_REQUIRE(op != SNB_DIFF_AUG_COLOR || (d->brightness && d->saturation && d->contrast),
+                "%s: the policy lists color but a color draw is NULL", who);
+    SNB_REQUIRE(op != SNB_DIFF_AUG_TRANSLATION || (d->translation_y && d->translation_x),
+                "%s: the policy lists translation but a translation draw is NULL", who);
+    SNB_REQUIRE(op != SNB_DIFF_AUG_CUTOUT || (d->cutout_y && d->cutout_x),
+                "%s: the policy lists cutout but a cutout draw is NULL", who);
+  }
+  if (int rc = check_patch_extents(who, n, channels, height, width, 1)) return rc;
+  SNB_REQUIRE((int64_t)n * height * width < (int64_t(1) << 31), "%s: %d images of %d x %d are too many pixels", who,
+              n, height, width);
+  if (int rc = check_nchw(who, "the source", src, ss)) return rc;
+  if (int rc = check_nchw(who, "the destination", dst, ds)) return rc;
+  SNB_REQUIRE(workspace != nullptr, "%s: null workspace", who);
+  return SNB_OK;
+}
+
 }  // namespace snb
 
 using namespace snb;
@@ -737,6 +768,30 @@ int snb_render_forward(const SnbRenderArgs* a, void* stream) {
                                          stream);
   return snb_composite_forward(a->raw_fine, 4, a->z_fine, a->rays, a->noise_fine, a->noise_std, a->white_back,
                                a->n_rays, S + Ni, a->rgb_fine, a->depth_fine, a->weights_fine, stream);
+}
+
+int snb_diff_augment_forward(const int* ops, int n_ops, const SnbDiffAugDraws* draws, const float* input,
+                             const int64_t* in_strides, int n, int channels, int height, int width, float* out,
+                             const int64_t* out_strides, float* workspace, void* stream) {
+  const char* who = "snb_diff_augment_forward";
+  if (int rc = check_diff_augment(who, ops, n_ops, draws, input, in_strides, n, channels, height, width, out,
+                                  out_strides, workspace))
+    return rc;
+  const SnbDiffAugDraws none{};
+  return launch_diff_augment(false, ops, n_ops, draws ? *draws : none, input, in_strides, n, channels, height, width,
+                             out, out_strides, workspace, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int snb_diff_augment_backward(const int* ops, int n_ops, const SnbDiffAugDraws* draws, const float* d_out,
+                              const int64_t* d_out_strides, int n, int channels, int height, int width, float* d_input,
+                              const int64_t* d_in_strides, float* workspace, void* stream) {
+  const char* who = "snb_diff_augment_backward";
+  if (int rc = check_diff_augment(who, ops, n_ops, draws, d_out, d_out_strides, n, channels, height, width, d_input,
+                                  d_in_strides, workspace))
+    return rc;
+  const SnbDiffAugDraws none{};
+  return launch_diff_augment(true, ops, n_ops, draws ? *draws : none, d_out, d_out_strides, n, channels, height,
+                             width, d_input, d_in_strides, workspace, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

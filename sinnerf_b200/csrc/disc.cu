@@ -1078,7 +1078,222 @@ int forward_args(const char* who, int imsize, int precision, const float* const*
   return SNB_OK;
 }
 
+// ------------------------------------------------------------------ standalone DiffAugment (snb_diff_augment_*)
+// Any policy, in its order, on (n, c, h, w) through strides.  Per image, 4 floats per op (the workspace):
+//   color:       brightness shift rand - 0.5, saturation factor 2 rand, contrast factor rand + 0.5, and the forward's
+//                contrast mean (rand_contrast's x_mean) or the backward's mean of the contrast's output gradient
+//   translation: row and column shift (the input pixel an output pixel reads is its own plus the shift)
+//   cutout:      the zeroed rows y0..y1 and columns x0..x1 (inclusive; rand_cutout's clamped index range)
+// A pixel's value after ops [0, k) is a function of one input pixel (or of none: a translation moved in padding) and
+// of per-pixel channel means, one per color op, which each thread recomputes for its own pixel: no pass stores an
+// intermediate image.  The color arithmetic is the expressions of aug_saturated and disc_gather_kernel, channel sum
+// in channel order, so 'color' followed by 'cutout' gives disc_gather_kernel's bits.
+constexpr int kDaMaxOps = SNB_DIFF_AUG_MAX_OPS, kDaFloats = SNB_DIFF_AUG_WS_FLOATS;
+static_assert(kDaFloats == 4 * kDaMaxOps, "4 workspace floats per op and image");
+
+struct DaArgs {
+  SnbDiffAugDraws d;
+  int n_ops, op[kDaMaxOps], row[kDaMaxOps];   // row: the op's occurrence among the policy's ops of its kind
+  int n, c, h, w, cut_h, cut_w;
+  const float* src; long long s_b, s_c, s_y, s_x;   // forward: the input; backward: the output gradient
+  float* dst; long long d_b, d_c, d_y, d_x;         // forward: the output; backward: the input gradient
+  float* ws;
+};
+
+// image b's draws as op parameters, the means left zero
+__device__ void da_params(const DaArgs& a, int b, float* q) {
+  auto clampi = [](long long v, int hi) { return (float)(v < 0 ? 0 : v > hi ? hi : v); };
+  for (int k = 0; k < a.n_ops; ++k) {
+    const long long r = (long long)a.row[k] * a.n + b;
+    float* p = q + 4 * k;
+    if (a.op[k] == SNB_DIFF_AUG_COLOR) {
+      p[0] = a.d.brightness[r] - 0.5f; p[1] = a.d.saturation[r] * 2.f; p[2] = a.d.contrast[r] + 0.5f; p[3] = 0.f;
+    } else if (a.op[k] == SNB_DIFF_AUG_TRANSLATION) {
+      p[0] = (float)a.d.translation_y[r]; p[1] = (float)a.d.translation_x[r]; p[2] = p[3] = 0.f;
+    } else {
+      const long long oy = a.d.cutout_y[r] - a.cut_h / 2, ox = a.d.cutout_x[r] - a.cut_w / 2;
+      p[0] = clampi(oy, a.h - 1); p[1] = clampi(oy + a.cut_h - 1, a.h - 1);
+      p[2] = clampi(ox, a.w - 1); p[3] = clampi(ox + a.cut_w - 1, a.w - 1);
+    }
+  }
+}
+
+__device__ __forceinline__ bool da_cut(const float* p, int y, int x) {
+  return (float)y >= p[0] && (float)y <= p[1] && (float)x >= p[2] && (float)x <= p[3];
+}
+
+// forward: where pixel (y, x) of the image after ops [0, k) comes from.  start: the first op its value goes through
+// (0: from the input at (y, x) as returned; j > 0: from the zero that op j - 1's translation read in the padding,
+// (y, x) then being its position after op j - 1)
+struct DaSrc { int start, y, x; };
+__device__ DaSrc da_trace(const DaArgs& a, const float* q, int k, int y, int x) {
+  for (int j = k - 1; j >= 0; --j) {
+    if (a.op[j] != SNB_DIFF_AUG_TRANSLATION) continue;
+    const int sy = y + (int)q[4 * j], sx = x + (int)q[4 * j + 1];
+    if (sy < 0 || sy >= a.h || sx < 0 || sx >= a.w) return {j + 1, y, x};
+    y = sy; x = sx;
+  }
+  return {0, y, x};
+}
+
+// channel c of that pixel after ops [s.start, k); m: its channel means of the color ops among them; px: its input
+__device__ float da_value(const DaArgs& a, const float* q, const float* m, DaSrc s, int k, const float* px, int c) {
+  float v = s.start == 0 ? px[c * a.s_c] : 0.f;
+  int y = s.y, x = s.x;
+  for (int j = s.start; j < k; ++j) {
+    const float* p = q + 4 * j;
+    if (a.op[j] == SNB_DIFF_AUG_COLOR) {
+      const float t = (v + p[0] - m[j]) * p[1] + m[j];
+      v = (t - p[3]) * p[2] + p[3];
+    } else if (a.op[j] == SNB_DIFF_AUG_TRANSLATION) {
+      y -= (int)p[0]; x -= (int)p[1];
+    } else if (da_cut(p, y, x)) {
+      v *= 0.f;
+    }
+  }
+  return v;
+}
+
+// m[j] for every color op j in [s.start, k): the channel mean of its brightened input at this pixel
+__device__ void da_means(const DaArgs& a, const float* q, DaSrc s, int k, const float* px, float* m) {
+  for (int j = s.start; j < k; ++j) {
+    if (a.op[j] != SNB_DIFF_AUG_COLOR) continue;
+    float acc = da_value(a, q, m, s, j, px, 0) + q[4 * j];
+    for (int c = 1; c < a.c; ++c) acc += da_value(a, q, m, s, j, px, c) + q[4 * j];
+    m[j] = acc / (float)a.c;
+  }
+}
+
+// backward: where the gradient with respect to pixel (y, x) of the image after ops [0, k) comes from.  end: the
+// stage it starts at (n_ops: the output gradient at (y, x) as returned; j < n_ops: zero, op j's translation moving
+// the pixel out, (y, x) then being its position before op j).  Color ops before that stage still pass it the
+// gradient of their image-wide mean.
+struct DaDst { int end, y, x; };
+__device__ DaDst da_to_output(const DaArgs& a, const float* q, int k, int y, int x) {
+  for (int j = k; j < a.n_ops; ++j) {
+    if (a.op[j] != SNB_DIFF_AUG_TRANSLATION) continue;
+    const int ny = y - (int)q[4 * j], nx = x - (int)q[4 * j + 1];
+    if (ny < 0 || ny >= a.h || nx < 0 || nx >= a.w) return {j, y, x};
+    y = ny; x = nx;
+  }
+  return {a.n_ops, y, x};
+}
+
+// channel c of the gradient with respect to the image after ops [0, k) at that pixel, through ops e.end - 1 .. k;
+// gp: its output gradient; nm: its channel means of the gradient at each of those color ops' saturation output
+__device__ float da_grad(const DaArgs& a, const float* q, const float* nm, int k, DaDst e, const float* gp, int c) {
+  float g = e.end == a.n_ops ? gp[c * a.s_c] : 0.f;
+  int y = e.y, x = e.x;
+  for (int j = e.end - 1; j >= k; --j) {
+    const float* p = q + 4 * j;
+    if (a.op[j] == SNB_DIFF_AUG_COLOR) {
+      g = p[2] * g + (1.f - p[2]) * p[3];
+      g = p[1] * g + (1.f - p[1]) * nm[j];
+    } else if (a.op[j] == SNB_DIFF_AUG_TRANSLATION) {
+      y += (int)p[0]; x += (int)p[1];
+    } else if (da_cut(p, y, x)) {
+      g *= 0.f;
+    }
+  }
+  return g;
+}
+
+__device__ void da_grad_means(const DaArgs& a, const float* q, int k, DaDst e, const float* gp, float* nm) {
+  for (int j = e.end - 1; j >= k; --j) {
+    if (a.op[j] != SNB_DIFF_AUG_COLOR) continue;
+    const float con = q[4 * j + 2], S = q[4 * j + 3];
+    float acc = con * da_grad(a, q, nm, j + 1, e, gp, 0) + (1.f - con) * S;
+    for (int c = 1; c < a.c; ++c) acc += con * da_grad(a, q, nm, j + 1, e, gp, c) + (1.f - con) * S;
+    nm[j] = acc / (float)a.c;
+  }
+}
+
+// one block (256 threads) per image: the parameters, then each color op's image-wide mean in policy order (forward:
+// of its saturated input, as disc_aug_params_kernel sums it) or in reverse order (backward: of its output gradient)
+template <bool kBwd>
+__global__ void __launch_bounds__(256) diff_aug_stats_kernel(const DaArgs a) {
+  __shared__ float q[kDaFloats], red[32];
+  const int b = blockIdx.x, P = a.h * a.w;
+  if (threadIdx.x == 0) da_params(a, b, q);
+  __syncthreads();
+  for (int i = 0; i < a.n_ops; ++i) {
+    const int k = kBwd ? a.n_ops - 1 - i : i;
+    if (a.op[k] != SNB_DIFF_AUG_COLOR) continue;
+    float acc = 0.f;
+    for (int t = threadIdx.x; t < P; t += blockDim.x) {
+      float m[kDaMaxOps];
+      if constexpr (kBwd) {
+        const DaDst e = da_to_output(a, q, k + 1, t / a.w, t % a.w);
+        const float* gp = a.src + b * a.s_b + e.y * a.s_y + e.x * a.s_x;
+        da_grad_means(a, q, k + 1, e, gp, m);
+        for (int c = 0; c < a.c; ++c) acc += da_grad(a, q, m, k + 1, e, gp, c);
+      } else {
+        const DaSrc s = da_trace(a, q, k, t / a.w, t % a.w);
+        const float* px = a.src + b * a.s_b + s.y * a.s_y + s.x * a.s_x;
+        da_means(a, q, s, k + 1, px, m);
+        for (int c = 0; c < a.c; ++c) acc += (da_value(a, q, m, s, k, px, c) + q[4 * k] - m[k]) * q[4 * k + 1] + m[k];
+      }
+    }
+    acc = block_sum(acc, red);
+    if (threadIdx.x == 0) q[4 * k + 3] = acc / ((float)a.c * a.h * a.w);
+    __syncthreads();
+  }
+  if (threadIdx.x < kDaFloats) a.ws[(long long)kDaFloats * b + threadIdx.x] = q[threadIdx.x];
+}
+
+// one thread per pixel, all its channels.  Forward: output pixel (y, x); backward: input pixel (y, x)
+template <bool kBwd>
+__global__ void __launch_bounds__(256) diff_aug_map_kernel(const DaArgs a) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int P = a.h * a.w;
+  if (t >= (long long)a.n * P) return;
+  const int b = (int)(t / P), p = (int)(t % P), y = p / a.w, x = p % a.w;
+  float q[kDaFloats], m[kDaMaxOps];
+  for (int i = 0; i < 4 * a.n_ops; ++i) q[i] = a.ws[(long long)kDaFloats * b + i];
+  float* o = a.dst + b * a.d_b + y * a.d_y + x * a.d_x;
+  if constexpr (kBwd) {
+    const DaDst e = da_to_output(a, q, 0, y, x);
+    const float* gp = a.src + b * a.s_b + e.y * a.s_y + e.x * a.s_x;
+    da_grad_means(a, q, 0, e, gp, m);
+    for (int c = 0; c < a.c; ++c) o[c * a.d_c] = da_grad(a, q, m, 0, e, gp, c);
+  } else {
+    const DaSrc s = da_trace(a, q, a.n_ops, y, x);
+    const float* px = a.src + b * a.s_b + s.y * a.s_y + s.x * a.s_x;
+    da_means(a, q, s, a.n_ops, px, m);
+    for (int c = 0; c < a.c; ++c) o[c * a.d_c] = da_value(a, q, m, s, a.n_ops, px, c);
+  }
+}
+
 }  // namespace
+
+// snb_diff_augment_forward / _backward after api.cu's checks: src -> dst through the strides (backward: the output
+// gradient -> the input gradient)
+int launch_diff_augment(bool backward, const int* ops, int n_ops, const SnbDiffAugDraws& draws, const float* src,
+                        const int64_t* ss, int n, int c, int h, int w, float* dst, const int64_t* ds, float* ws,
+                        cudaStream_t st) {
+  DaArgs a{};
+  a.d = draws;
+  a.n_ops = n_ops;
+  int seen[3] = {0, 0, 0};
+  for (int k = 0; k < n_ops; ++k) { a.op[k] = ops[k]; a.row[k] = seen[ops[k]]++; }
+  a.n = n; a.c = c; a.h = h; a.w = w;
+  a.cut_h = (int)(h * 0.5 + 0.5); a.cut_w = (int)(w * 0.5 + 0.5);
+  a.src = src; a.s_b = ss[0]; a.s_c = ss[1]; a.s_y = ss[2]; a.s_x = ss[3];
+  a.dst = dst; a.d_b = ds[0]; a.d_c = ds[1]; a.d_y = ds[2]; a.d_x = ds[3];
+  a.ws = ws;
+  const unsigned blocks = (unsigned)(((long long)n * h * w + 255) / 256);
+  if (backward) {
+    diff_aug_stats_kernel<true><<<n, 256, 0, st>>>(a);
+    DISC_TRY(check_launch("diff_aug_stats_kernel"));
+    diff_aug_map_kernel<true><<<blocks, 256, 0, st>>>(a);
+    return check_launch("diff_aug_map_kernel");
+  }
+  diff_aug_stats_kernel<false><<<n, 256, 0, st>>>(a);
+  DISC_TRY(check_launch("diff_aug_stats_kernel"));
+  diff_aug_map_kernel<false><<<blocks, 256, 0, st>>>(a);
+  return check_launch("diff_aug_map_kernel");
+}
+
 }  // namespace snb
 
 using namespace snb;

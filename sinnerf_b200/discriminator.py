@@ -25,6 +25,11 @@ The GEMM arithmetic follows `precision=` or the process setting (config.resolve_
 sinnerf_b200.vit: the fp16 hi + lo three-product split by default, 'f16' / 'bf16' single products, and under
 'autocast' fp16 autocast gives 'f16', the arithmetic of the reference's cuDNN convolutions under Lightning's
 precision=16.  There is no CPU path.
+
+`DiffAugment(x, policy, channels_first)` is models/diff_aug.py's standalone augmentation (any policy, translation
+included) on the library's kernels, for dloss='relavistic''s `self.D(DiffAugment(real_patch))`:
+
+    from sinnerf_b200.discriminator import DiffAugment        # models/sinnerf.py:14
 """
 from __future__ import annotations
 
@@ -38,7 +43,7 @@ from torch.autograd.function import once_differentiable
 from . import _lib
 from .config import resolve_precision
 
-__all__ = ["Discriminator", "layer_schedule", "output_sizes", "draw_augment"]
+__all__ = ["Discriminator", "DiffAugment", "layer_schedule", "output_sizes", "draw_augment", "diff_augment_draws"]
 
 POLICIES = (None, "", "color,cutout")
 
@@ -77,22 +82,53 @@ def output_sizes(imsize, h: int, w: int):
     return sizes
 
 
+def _draw_color(B, H, W, device):
+    # rand_brightness, rand_saturation, rand_contrast
+    return tuple(torch.rand(B, 1, 1, 1, dtype=torch.float32, device=device).reshape(B) for _ in range(3))
+
+
+def _draw_translation(B, H, W, device):
+    # rand_translation: the shifts of dim 2 (rows) and of dim 3 (columns)
+    sy, sx = int(H * 0.125 + 0.5), int(W * 0.125 + 0.5)
+    ty = torch.randint(-sy, sy + 1, size=[B, 1, 1], device=device)
+    tx = torch.randint(-sx, sx + 1, size=[B, 1, 1], device=device)
+    return ty.reshape(B), tx.reshape(B)
+
+
+def _draw_cutout(B, H, W, device):
+    # rand_cutout: the offsets along the rows and the columns
+    ch, cw = int(H * 0.5 + 0.5), int(W * 0.5 + 0.5)
+    oy = torch.randint(0, H + (1 - ch % 2), size=[B, 1, 1], device=device)
+    ox = torch.randint(0, W + (1 - cw % 2), size=[B, 1, 1], device=device)
+    return oy.reshape(B), ox.reshape(B)
+
+
+_DRAWS = {"color": _draw_color, "translation": _draw_translation, "cutout": _draw_cutout}
+
+
+def diff_augment_draws(policy, shape, device):
+    """The random draws of models/diff_aug.py DiffAugment(x, policy) for x of shape (B, C, H, W), made with the same
+    calls in the same order: its gate np.random.random() < 0.5 gives None (DiffAugment returns x), else the list
+    [(op, draws)] over the policy's ops in order -- empty for an empty or None policy -- with draws (brightness,
+    saturation, contrast), (row shift, column shift) or (cutout row offset, cutout column offset), each of (B,)
+    device tensors.  An unknown op raises KeyError once the draws before it are made, as AUGMENT_FNS[p] does."""
+    if np.random.random() < 0.5:
+        return None
+    B, _, H, W = shape
+    return [(p, _DRAWS[p](B, H, W, device)) for p in policy.split(",")] if policy else []
+
+
 def draw_augment(policy, shape, device):
     """The random draws of Discriminator.forward + DiffAugment (models/discriminator.py:159, models/diff_aug.py),
     made with the same calls in the same order: None when no augmentation applies, else the tuple (brightness,
     saturation, contrast, cutout row offset, cutout column offset) of (B,) device tensors."""
     if policy is None or not np.random.random() > 0.5:
         return None
-    if np.random.random() < 0.5 or not policy:
+    draws = diff_augment_draws(policy, shape, device)
+    if not draws:
         return None
-    B, _, H, W = shape
-    ch, cw = int(H * 0.5 + 0.5), int(W * 0.5 + 0.5)
-    rb = torch.rand(B, 1, 1, 1, dtype=torch.float32, device=device)
-    rs = torch.rand(B, 1, 1, 1, dtype=torch.float32, device=device)
-    rc = torch.rand(B, 1, 1, 1, dtype=torch.float32, device=device)
-    oy = torch.randint(0, H + (1 - ch % 2), size=[B, 1, 1], device=device)
-    ox = torch.randint(0, W + (1 - cw % 2), size=[B, 1, 1], device=device)
-    return tuple(t.reshape(B) for t in (rb, rs, rc, oy, ox))
+    (_, color), (_, cutout) = draws
+    return color + cutout
 
 
 def _ptrs(ts):
@@ -255,3 +291,91 @@ class Discriminator(nn.Module):
         """
         cfg, weights = self._call_args(input, "Discriminator.forward_with_penalty")
         return _PenaltyFn.apply(cfg, input, *weights)
+
+
+class _DiffAugFn(torch.autograd.Function):
+    """DiffAugment's ops with the given draws; backward to x through the same draws"""
+
+    @staticmethod
+    def forward(ctx, x, channels_first, draws):
+        lib = _lib.load()
+        if channels_first:
+            B, Ch, H, W = x.shape
+            out = torch.empty(B, Ch, H, W, device=x.device, dtype=torch.float32)
+        else:
+            B, H, W, Ch = x.shape
+            out = torch.empty(B, H, W, Ch, device=x.device, dtype=torch.float32)
+        ops, d, _ = _diff_aug_args(draws, B)
+        ws = torch.empty(B * _lib.DIFF_AUG_WS_FLOATS, device=x.device, dtype=torch.float32)
+        _lib.check(lib.snb_diff_augment_forward(ops, len(draws), C.byref(d), _lib.ptr(x), _nchw_strides(x, channels_first),
+                                                B, Ch, H, W, _lib.ptr(out), _nchw_strides(out, channels_first),
+                                                _lib.ptr(ws), _lib.stream_ptr(x.device)), "snb_diff_augment_forward")
+        # the gradient's layout: x's strides where empty_like keeps them (a permuted view stays permuted)
+        ctx.args = (channels_first, draws, (B, Ch, H, W), torch.empty_like(x, device="meta"))
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        channels_first, draws, (B, Ch, H, W), like = ctx.args
+        if not ctx.needs_input_grad[0]:
+            return None, None, None
+        lib = _lib.load()
+        g = g.detach().to(torch.float32)
+        dx = torch.empty_strided(like.shape, like.stride(), device=g.device, dtype=torch.float32)   # all written
+        ops, d, _ = _diff_aug_args(draws, B)
+        ws = torch.empty(B * _lib.DIFF_AUG_WS_FLOATS, device=g.device, dtype=torch.float32)
+        _lib.check(lib.snb_diff_augment_backward(ops, len(draws), C.byref(d), _lib.ptr(g), _nchw_strides(g, channels_first),
+                                                 B, Ch, H, W, _lib.ptr(dx), _nchw_strides(dx, channels_first),
+                                                 _lib.ptr(ws), _lib.stream_ptr(g.device)), "snb_diff_augment_backward")
+        return dx, None, None
+
+
+def _nchw_strides(t, channels_first):
+    """t's element strides in (image, channel, row, column) order"""
+    s = t.stride()
+    return (C.c_int64 * 4)(*(s if channels_first else (s[0], s[3], s[1], s[2])))
+
+
+def _diff_aug_args(draws, B):
+    """(op codes, SnbDiffAugDraws, the tensors it points into): an op's k-th occurrence reads row k of its draws"""
+    fields = {"color": ("brightness", "saturation", "contrast"), "translation": ("translation_y", "translation_x"),
+              "cutout": ("cutout_y", "cutout_x")}
+    rows = {}
+    for op, ts in draws:
+        rows.setdefault(op, []).append(ts)
+    d, keep = _lib.SnbDiffAugDraws(), []
+    for op, occ in rows.items():
+        for name, ts in zip(fields[op], zip(*occ)):
+            t = ts[0] if len(ts) == 1 else torch.stack(ts)
+            keep.append(t)
+            setattr(d, name, t.data_ptr())
+    ops = (C.c_int * max(len(draws), 1))(*[_lib.DIFF_AUG_OPS[op] for op, _ in draws])
+    return ops, d, keep
+
+
+def DiffAugment(x, policy="color,cutout", channels_first=True):
+    """models/diff_aug.py DiffAugment(x, policy, channels_first) on the library's kernels (csrc/disc.cu).
+
+    x: fp32 CUDA (B, C, H, W), or (B, H, W, C) with channels_first=False, any C >= 1, read through its strides (a
+    permuted view is not copied).  The reference's draws are made with the same calls in the same order (see
+    diff_augment_draws): on its gate, or for an empty or None policy, x itself is returned; otherwise a new
+    contiguous tensor of x's shape, with the policy's ops ('color', 'translation', 'cutout', in the order given)
+    applied, and an unknown op raises KeyError.  The arithmetic is fp32 whatever the autocast state or precision
+    setting, and where the policy is 'color,cutout' the values are the ones Discriminator(policy='color,cutout')
+    feeds its first convolution for the same draws, bit for bit.  Differentiable in x, once: the gradient comes back
+    with x's strides.  Nothing synchronises with the host."""
+    if not isinstance(x, torch.Tensor):
+        raise TypeError(f"DiffAugment: input is not a torch.Tensor (got {type(x)})")
+    if x.dim() != 4 or min(x.shape) < 1:
+        raise ValueError(f"DiffAugment: invalid input shape, we expect a non-empty 4-d tensor. Got: {tuple(x.shape)}")
+    _lib.require_device(x, "DiffAugment")
+    if x.dtype != torch.float32:
+        raise TypeError(f"DiffAugment: input must be float32 (got {x.dtype})")
+    B, Ch, H, W = x.shape if channels_first else (x.shape[0], x.shape[3], x.shape[1], x.shape[2])
+    draws = diff_augment_draws(policy, (B, Ch, H, W), x.device)
+    if not draws:
+        return x
+    if len(draws) > _lib.DIFF_AUG_MAX_OPS:
+        raise ValueError(f"DiffAugment: policy {policy!r} has {len(draws)} ops, more than {_lib.DIFF_AUG_MAX_OPS}")
+    return _DiffAugFn.apply(x, bool(channels_first), draws)
