@@ -98,7 +98,7 @@ struct DiscWs {
   // gradient penalty (pen = 1): g = grad_x sum(out) (n, 3, h, w), the tangent direction v, its DiffAugment
   // parameters, each layer's tangent im2col and pre-norm tangent output with its InstanceNorm statistics, the
   // primal-adjoint stream's scratch and both streams' raw weight gradients
-  float *g, *ones, *vt, *taug, *dp0, *dp1, *dcolp;
+  float *g, *ones, *vt, *taug, *dreg, *dp0, *dp1, *dcolp;   // dreg: d_reg 2^-ev[0] (see disc_pen_dir_kernel)
   float *tcol[kMaxLayers], *ty[kMaxLayers], *tmean[kMaxLayers], *tq[kMaxLayers], *dwt[kMaxLayers], *dwp[kMaxLayers];
   int *ev, *gt, *gp, *gu, *gw;    // per layer: exponents of the tangent col, of both adjoint streams, of a fold's
                                   // primal output and of the combined weight gradient
@@ -132,6 +132,7 @@ DiscWs disc_ws(void* base, const Net& N, int save, int pen = 0) {
     const long long img = 3ll * N.n * N.h * N.w;
     W.g = take(img); W.vt = take(img); W.ones = take((long long)N.n * N.l[N.n_layers - 1].P());
     W.taug = take((long long)kAugFloats * N.n);
+    W.dreg = take(N.n);
     W.dp0 = take(dy_max); W.dp1 = take(dy_max); W.dcolp = take(dcol_max);
     int* e = reinterpret_cast<int*>(take(5 * kMaxLayers));
     W.ev = e; W.gt = e + kMaxLayers; W.gp = e + 2 * kMaxLayers; W.gu = e + 3 * kMaxLayers; W.gw = e + 4 * kMaxLayers;
@@ -569,11 +570,14 @@ __global__ void disc_fold2_kernel(const Fold2Args a) {
   if (blockIdx.x == 0 && threadIdx.x == 0) *a.e_out = ex;
 }
 
-// v = 2 d_reg[b] g[b] (n, 3, h, w): the tangent direction whose Hessian-vector product is the penalty's gradient
-__global__ void disc_pen_dir_kernel(const float* __restrict__ g, const float* __restrict__ d_reg, long long per_image,
+// v = 2 d_reg[b] g[b] (n, 3, h, w): the tangent direction whose Hessian-vector product is the penalty's gradient.
+// dreg is d_reg scaled by the power of two that puts its largest element in [2^14, 2^15), the exponent carried in
+// ev[0]: as a float factor, a small d_reg (2^-126 times integers below 2^10) made v subnormal or 0 before its own
+// rescale, and a large one could overflow it
+__global__ void disc_pen_dir_kernel(const float* __restrict__ g, const float* __restrict__ dreg, long long per_image,
                                     long long m, float* __restrict__ v) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < m) v[i] = 2.f * d_reg[i / per_image] * g[i];
+  if (i < m) v[i] = 2.f * dreg[i / per_image] * g[i];
 }
 
 __global__ void disc_fill_kernel(float* __restrict__ x, long long m, float v) {
@@ -912,9 +916,11 @@ int disc_penalty_backward_impl(const Net& N, const float* const* W, const float*
   if (!any) return SNB_OK;
   const long long img = 3ll * N.n * N.h * N.w, P0 = (long long)N.h * N.w;
   // tangent forward along v, each layer's tangent col scaled to [2^14, 2^15) with its exponent in ev
-  disc_pen_dir_kernel<<<blocks_of(img, 256), 256, 0, st>>>(ws.g, d_reg, 3 * P0, img, ws.vt);
+  disc_grad_scale_kernel<<<1, 1024, 0, st>>>(d_reg, N.n, ws.dreg, nullptr, ws.ev);
+  DISC_TRY(check_launch("disc_grad_scale_kernel"));
+  disc_pen_dir_kernel<<<blocks_of(img, 256), 256, 0, st>>>(ws.g, ws.dreg, 3 * P0, img, ws.vt);
   DISC_TRY(check_launch("disc_pen_dir_kernel"));
-  disc_grad_scale_kernel<<<1, 1024, 0, st>>>(ws.vt, img, ws.vt, nullptr, ws.ev);
+  disc_grad_scale_kernel<<<1, 1024, 0, st>>>(ws.vt, img, ws.vt, ws.ev, ws.ev);
   DISC_TRY(check_launch("disc_grad_scale_kernel"));
   disc_aug_tangent_params_kernel<<<N.n, 256, 0, st>>>(ws.vt, N.h, N.w, ws.aug, ws.taug);
   DISC_TRY(check_launch("disc_aug_tangent_params_kernel"));
